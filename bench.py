@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- TPC-H Q1 / Q6 lineitem scan + filter + partial aggregate on N B200s vs the CPU path.
+"""bench.py -- TPC-H Q1 / Q6 lineitem scan + filter + partial aggregate on N H100s vs the CPU path.
 
-Contract (see the task brief): `python bench.py --gpus N --steps K --warmup W` (under torchrun for
-N > 1) prints ONE JSON line on rank 0.  A "step" is one execution of the query over the whole
+Usage: `python bench.py --gpus N --steps K --warmup W` (under torchrun for N > 1) prints ONE JSON line on
+rank 0.  A "step" is one execution of the query over the whole
 (sharded) column table:
 
   value   whole-job rows/s with the ColumnBatches resident in HBM (sd_plan_scan_store), including the
@@ -28,6 +28,10 @@ partition set instead.  Q6 over SF-10 is measured in the same run and reported u
 `parity_check`: in the same run the oracle's generated-loop layer (CPU) scans the SAME ColumnBatch bytes at the
 benchmark's own size (every rank its shard; partial rows gathered and merged) and the GPU result must match: counts
 bit-exact, DOUBLE sums / averages within 1e-6 relative (BASELINE.json north_star).  A mismatch fails the run.
+
+`--dump-outputs DIR` writes the final rows of the last timed step of each query (Q1 and Q6) as DIR/q1_final_rows.npy and
+DIR/q6_final_rows.npy (float64, one row per group, sorted by key).  The tables are generated from fixed seeds, so two builds
+run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -70,16 +74,9 @@ def parse_args():
                     help="N > 1: strong (default, BASELINE.json: ONE SF-100 table over 1->8 GPUs) = the table split into N contiguous "
                          "batch ranges, one partition set per GPU; weak = every rank scans its own table-sized partition set")
     ap.add_argument("--no-parity", action="store_true", help="skip the GPU-vs-oracle parity check at the benchmark's own size")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the final rows of each timed query's last step as DIR/<name>.npy (float64)")
     return ap.parse_args()
-
-
-def ncu_traffic_per_row(q1):
-    """DRAM bytes per row of the scan kernel from the committed `ncu --set full` capture (profiles/)."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))["q1" if q1 else "q6"]
-        return (t["dram_read_bytes"] + t["dram_write_bytes"]) / t["rows"]
-    except Exception:
-        return None
 
 
 def measured_peak_gbs():
@@ -87,7 +84,7 @@ def measured_peak_gbs():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 def cgroup_cpu_limit():
@@ -239,7 +236,7 @@ def workload_config(q1, total, gpus, scaling="weak"):
             "total_rows": total * gpus if scaling == "weak" else total,
             "rows_per_batch": ROWS_PER_BATCH, "bytes_per_row": 40 if q1 else 28,
             "sharding": sharding,
-            "l2": "inputs per step (>= 3 GB per GPU) are larger than the 126 MB L2; no flush needed",
+            "l2": "inputs per step (>= 3 GB per GPU) are larger than the 50 MB L2; no flush needed",
             "literals": "Q1 cutoff 1997-10-02; Q6 1994-01-01, 0.05..0.07, 24"}
 
 
@@ -354,39 +351,38 @@ class QueryRun:
         lz.LZ4_compressBound.restype = C.c_int
         lz.LZ4_compressBound.argtypes = [C.c_int]
         cols = self.desc.table_cols
-        jobs, off = [], 0
-        for bi, mb in enumerate(self.marshalled):
-            for k, c in enumerate(cols):
-                n = int(mb.col_lens[k])
-                cap = lz.LZ4_compressBound(n) + 8
-                jobs.append((bi, k, int(mb.col_bufs[k]), n, off, cap))
-                off += (cap + 63) // 64 * 64
-        arena = torch.empty(max(off, 64), dtype=torch.uint8).pin_memory()
-        base = arena.data_ptr()
+        jobs = [(bi, k, int(mb.col_bufs[k]), int(mb.col_lens[k])) for bi, mb in enumerate(self.marshalled) for k in range(len(cols))]
+        # one compressBound-sized scratch per thread; only the accepted envelopes are kept, each in an array of its own size
+        # (a scratch slot per buffer would make another full copy of the table resident: 24 GB at SF-100)
+        scratch = threading.local()
 
         def work(j):
-            bi, k, src, n, o, cap = j
+            bi, k, src, n = j
             if n < 2048:
-                return (bi, k, src, n)
-            cl = lz.LZ4_compress_default(src, base + o + 8, n, cap - 8)
+                return (bi, k, src, n, None)
+            cap = lz.LZ4_compressBound(n)
+            buf = getattr(scratch, "buf", None)
+            if buf is None or len(buf) < cap + 8:
+                buf = scratch.buf = np.empty(cap + 8, dtype=np.uint8)
+            cl = lz.LZ4_compress_default(src, buf.ctypes.data + 8, n, cap)
             if cl <= 0 or cl > (n * 3) // 4:
-                return (bi, k, src, n)
-            hdr = np.frombuffer((C.c_char * 8).from_address(base + o), dtype="<i4")
-            hdr[0], hdr[1] = -1, n
-            return (bi, k, base + o, cl + 8)
+                return (bi, k, src, n, None)
+            buf[:8].view("<i4")[:] = (-1, n)
+            env = buf[:cl + 8].copy()
+            return (bi, k, env.ctypes.data, cl + 8, env)
         with concurrent.futures.ThreadPoolExecutor(max_workers=threads) as ex:
             res = list(ex.map(work, jobs, chunksize=64))
         # the stored buffers back to back (64-byte aligned) in one pinned arena, batch after batch -- the layout of the plain
-        # host copy above; the scratch arena with compressBound-sized slots is dropped
-        tight_total = sum((ln + 63) // 64 * 64 for _, _, _, ln in res)
-        tight = torch.empty(max(tight_total, 64), dtype=torch.uint8).pin_memory()
+        # host copy above
+        tight_total = sum((ln + 63) // 64 * 64 for _, _, _, ln, _ in res)
+        tight = torch.empty(max(tight_total, 64), dtype=torch.uint8, pin_memory=True)
         tbase, toff = tight.data_ptr(), 0
         moved = []
-        for bi, k, ptr, ln in res:
+        for bi, k, ptr, ln, _ in res:
             C.memmove(tbase + toff, ptr, ln)
             moved.append((bi, k, tbase + toff, ln))
             toff += (ln + 63) // 64 * 64
-        del arena
+        del res
         self.host_keep.append(tight)
         per_batch = {}
         for bi, k, ptr, ln in moved:
@@ -567,6 +563,27 @@ class QueryRun:
                 "oracle": [[x.decode() if isinstance(x, bytes) else x for x in r] for r in want[:8]]}
 
 
+def rows_array(rows, nkeys):
+    """Final rows -> float64 array (one row per group, sorted by the group keys).  STRING keys become the big-endian
+    integer of their first 6 bytes (exact in a double), NULLs become NaN."""
+    import numpy as np
+
+    def num(x):
+        if x is None:
+            return float("nan")
+        if isinstance(x, bytes):
+            return float(int.from_bytes(x[:6].ljust(6, b"\0"), "big"))
+        return float(x)
+    rows = sorted(rows, key=lambda r: tuple(num(x) for x in r[:nkeys]))
+    return np.array([[num(x) for x in r] for r in rows], dtype=np.float64).reshape(len(rows), -1)
+
+
+def dump_outputs(out_dir, name, rows, nkeys):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, name + ".npy"), rows_array(rows, nkeys))
+
+
 def timed_steps(torch, dist, world, fn, warmup, steps):
     for _ in range(warmup):
         fn()
@@ -660,6 +677,8 @@ def main():
     launches_timed = main_run.launches * args.steps // nsteps_all
     d2h_step = 0
     final_rows = capi.parse_row_stream(main_run.final_raw, main_run.desc.final_schema())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "q1_final_rows" if q1 else "q6_final_rows", final_rows, 2 if q1 else 0)
 
     out = {"metric": metric_name(q1), "value": job_rows * args.steps / (ms / 1e3), "unit": "rows/s", "n_gpus": world,
            "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True,
@@ -667,12 +686,11 @@ def main():
            "config": workload_config(q1, total, world, args.scaling), "gpu_launches": launches_timed, "clocks": clocks}
     peak, peak_src = measured_peak_gbs()
     achieved = algo_per_launch / (kernel_ms / 1e3) / 1e9 if kernel_ms > 0 else 0.0
-    tpr = ncu_traffic_per_row(q1)
     out["roofline"] = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                       "traffic": (tpr * main_run.local_rows) if tpr else None,
-                       "traffic_source": "profiles/r02_traffic.json (ncu --set full, 200M-row launch) scaled by rows", "peak_source": peak_src, "kernel": "sd::scan_aggregate_kernel<" + main_run.plan.kernel_name() + ">",
+                       "traffic": None, "traffic_source": "not measured", "peak_source": peak_src,
+                       "kernel": "sd::scan_aggregate_kernel<" + main_run.plan.kernel_name() + ">",
                        "kernel_ms_per_launch": kernel_ms, "algorithmic_bytes_per_launch": algo_per_launch,
-                       "frac_of_nominal_7700": achieved / 7700.0,
+                       "frac_of_datasheet_3350": achieved / 3350.0,
                        "note": "per rank (rank 0); one launch scans the rank's whole shard; `peak` is a measured COPY bandwidth "
                                "(read + write), which a read-only stream like this scan can exceed: frac > 1 is not an error"}
     out["hbm_gbs_whole_job"] = job_rows * (40 if q1 else 28) / (ms / args.steps / 1e3) / 1e9
@@ -760,6 +778,9 @@ def main():
         other = QueryRun(api, torch, dist, oq1, ototal, rank, world, local_rank, args.scaling, comm)
         oms = timed_steps(torch, dist, world, other.step_resident, args.warmup, args.steps)
         okms = other.kernel_ns / 1e6 / max(1, other.launches)
+        ofinal = capi.parse_row_stream(other.final_raw, other.desc.final_schema())
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, "q1_final_rows" if oq1 else "q6_final_rows", ofinal, 2 if oq1 else 0)
         oalgo = other.algo_bytes / max(1, other.launches)
         out["also"] = {"workload": workload_config(oq1, ototal, world, args.scaling)["workload"], "value": other.job_rows * args.steps / (oms / 1e3),
                        "unit": "rows/s", "ms_per_step": oms / args.steps,
@@ -767,7 +788,6 @@ def main():
                                     "unit": "GB/s", "frac": (oalgo / (okms / 1e3) / 1e9 / peak) if okms > 0 else 0.0,
                                     "kernel_ms_per_launch": okms}}
         if not args.no_parity:
-            ofinal = capi.parse_row_stream(other.final_raw, other.desc.final_schema())
             other.prepare_host_copy()
             other.step_e2e()
             out["also"]["parity_check"] = run_parity(other, "q1 sf100" if oq1 else "q6 sf10", ofinal)

@@ -1,5 +1,5 @@
 /*
- * snappy_gpu.h -- C ABI of libsnappygpu.so, the B200-native replacement for the inside of
+ * snappy_gpu.h -- C ABI of libsnappygpu.so, the H100-native replacement for the inside of
  * SnappyData's partial-aggregation stage:
  *
  *     ColumnTableScan -> [FilterExec / ProjectExec] -> SnappyHashAggregateExec(Partial)

@@ -1,9 +1,9 @@
-"""snappydata_b200 -- B200-native scan/decode/filter/partial-aggregate engine for
+"""snappydata_b200 -- H100-native (sm_90a) scan/decode/filter/partial-aggregate engine for
 SnappyData's column-store read path (see DESIGN.md).
 
 Only what the hot path needs lives here:
 
-  csrc/            CUDA kernels (sm_100a) + the C-ABI shared library (libsnappygpu.so)
+  csrc/            CUDA kernels (sm_90a) + the C-ABI shared library (libsnappygpu.so)
   column_format    host-side ColumnBatch byte-format writer/reader (the reference's
                    ColumnEncoding layouts), used to build fixtures and synthetic tables
   lineitem         synthetic TPC-H lineitem-shaped column tables (counter-based generator,

@@ -1,6 +1,6 @@
 // sd_codegen.cpp -- plan analysis + generation of the PLAN struct consumed by sd_kernels.cuh.
 //
-// This is the B200 counterpart of what the reference does in CodegenSupport.doProduce/doConsume:
+// This is the CUDA counterpart of what the reference does in CodegenSupport.doProduce/doConsume:
 // the reference emits Java for Janino per plan (ColumnTableScan.scala:186-672,
 // SnappyHashAggregateExec.scala:240-263, 450-491, 1278-1580); we emit a ~30-line CUDA struct that
 // plugs the plan's expressions into the hand-written kernel template.  The same generator feeds the
@@ -750,8 +750,8 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
     out.lit_nullable = o.lit_nullable ? 1 : 0;
     out.slow_paths = o.slow_paths ? 1 : 0;
     out.rpt = 4;
-    // group tables want the SM's shared memory; otherwise 2 CTAs per SM (sweep in profiles/r01_tuning.txt: Q6 6.9 TB/s
-    // at 2 vs 6.8 at 3, 6.5 at 1), 3 only for very narrow rows whose tiles are too small to keep enough bytes in flight
+    // group tables want the SM's shared memory; otherwise 2 CTAs per SM (H100 sweep, DESIGN.md section 5: Q6 at 2 is level
+    // with 1 and ahead of 3), 3 only for very narrow rows whose tiles are too small to keep enough bytes in flight
     out.min_ctas = out.mode == MODE_GROUPS ? 1 : (row_bytes <= 8 ? 3 : 2);
     out.stages = 1;
     if (const char* e = getenv("SD_TUNE_RPT")) { int v = atoi(e); if (v == 2 || v == 4 || v == 8) out.rpt = v; }

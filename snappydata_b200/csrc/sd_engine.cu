@@ -1440,7 +1440,7 @@ int sd_init(int device) {
   return 0;
 }
 int sd_device_count(int* out) { SD_CUDA(cudaGetDeviceCount(out)); return 0; }
-const char* sd_version(void) { return "snappydata_b200 0.1.0 (sm_100a)"; }
+const char* sd_version(void) { return "snappydata_b200 0.1.0 (sm_90a)"; }
 
 int sdx_stats_pass(const sd_plan_desc* desc, const sd_literal* lits, int32_t nlits, const void* stats, int64_t stats_len,
                    int32_t stats_ncols, int32_t num_rows, int32_t* pass) {
@@ -1487,7 +1487,7 @@ int sd_plan_create(const sd_plan_desc* desc, sd_plan** out) {
   p->lits.resize(p->spec.literal_types.size());
   p->lit_strs.resize(p->spec.literal_types.size());
   for (size_t i = 0; i < p->lits.size(); i++) { memset(&p->lits[i], 0, sizeof(sd_literal)); p->lits[i].type = p->spec.literal_types[i]; }
-  if (p->spec.mode == MODE_GROUPS) p->chunk_rows = 2 * CHUNK_ROWS;   // measured: tools/sweep.sh, profiles/r01_tuning.txt
+  if (p->spec.mode == MODE_GROUPS) p->chunk_rows = 2 * CHUNK_ROWS;   // tools/sweep.sh measures it
   if (const char* e = getenv("SD_TUNE_CHUNK_ROWS")) { int v = atoi(e); if (v >= 2048 && v % 2048 == 0 && v <= (1 << 20)) p->chunk_rows = v; }
   p->lits_set = p->lits.empty();
   *out = p.release();

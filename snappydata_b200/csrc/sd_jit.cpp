@@ -2,7 +2,7 @@
 // compiled kernel.  Mirrors the role Janino plays for the reference (WholeStageCodegen compiles the
 // generated class at plan time, caches it per plan: core/SnappySession.scala:2571-2607 plan cache):
 // generated PLAN struct + the hand-written kernel template (embedded as text) -> NVRTC -> cubin
-// for sm_100a -> CUfunction, cached in the kernel registry by plan signature.
+// for sm_90a -> CUfunction, cached in the kernel registry by plan signature.
 //
 // libnvrtc / libcuda are dlopen'ed on first use so that libsnappygpu.so itself loads on a box with no
 // driver (the CPU-only build/test container).
@@ -124,7 +124,7 @@ int jit_compile(const PlanSpec& spec, int device, KernelEntry& out) {
   if (nr != NVRTC_SUCCESS) return set_error(SD_ERR_CUDA, "nvrtcCreateProgram: %s", d.GetErrorString(nr));
   d.AddNameExpression(prog, name_expr.c_str());
   // -lineinfo adds ~50 % to the compile: only when a profile of a JIT kernel is wanted (SD_JIT_LINEINFO=1)
-  std::vector<std::string> optv = {"--gpu-architecture=sm_100a", "-std=c++17", "--fmad=false", "-default-device"};
+  std::vector<std::string> optv = {"--gpu-architecture=sm_90a", "-std=c++17", "--fmad=false", "-default-device"};
   const char* li = getenv("SD_JIT_LINEINFO");
   if (li && atoi(li) > 0) optv.push_back("-lineinfo");
   if (const char* defs = getenv("SD_JIT_DEFINES")) {   // space-separated -DNAME=VALUE switches (experiments; part of the plan signature)

@@ -1,7 +1,7 @@
-// sd_kernels.cuh -- the fused scan -> decode -> filter -> partial-aggregate kernel for sm_100a.
+// sd_kernels.cuh -- the fused scan -> decode -> filter -> partial-aggregate kernel for sm_90a.
 //
 // One kernel template, specialised per plan by a small generated struct (PLAN) that supplies the
-// plan's column kinds and three inline functions: filter(), group() and slots() -- the B200
+// plan's column kinds and three inline functions: filter(), group() and slots() -- the CUDA
 // counterpart of the reference's WholeStageCodegen class for
 //   ColumnTableScan.doProduce            core/execution/columnar/ColumnTableScan.scala:186-672
 //   FilterExec.doConsume                 (Spark 2.1.1)
@@ -17,7 +17,7 @@
 //     cache-streaming vector load per row pair per lane (16/8/4/2 bytes per lane);
 //   * all loads of a tile (every column, RPT rows) are issued before the first use, so each thread
 //     keeps NC * RPT/2 independent requests in flight;
-//   * a persistent grid of 148 * CTAS_PER_SM CTAs walks (batch, chunk) work items round-robin -- no
+//   * a persistent grid of num_SMs * CTAS_PER_SM CTAs walks (batch, chunk) work items round-robin -- no
 //     per-batch launch, deterministic reduction order;
 //   * aggregation never touches global atomics on the hot path: registers (no keys) or per-thread
 //     private shared-memory tables laid out bank-conflict free (small group counts), reduced once per
@@ -1112,7 +1112,7 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
           // and will be refilled through the ASYNC proxy (cp.async.bulk): the mbarrier alone does not order the two (PTX ISA, "async
           // proxy": accesses to the same location across proxies need a cross-proxy fence).  Without the fence a refill can land
           // while loads issued before the release are still pending -- seen when the LSU is busy with a hash plan's global
-          // atomics: ~1 % of the staged values then belong to the stage's NEXT tile (profiles/r02_ring_proxy_fence.txt).
+          // atomics: ~1 % of the staged values then belong to the stage's NEXT tile.
 #ifndef SD_EXP_NO_PROXY_FENCE   // (diagnostic builds reproduce the failure with -DSD_EXP_NO_PROXY_FENCE)
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 #endif

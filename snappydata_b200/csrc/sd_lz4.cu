@@ -105,7 +105,7 @@ int decompress_envelope_host(const uint8_t* buf, int64_t len, std::vector<uint8_
 // A column buffer is ONE LZ4 block (the reference compresses the whole value, CompressionUtils.scala:102-110), so
 // the unit of independent work is the buffer and the time of a launch is the serial chain of its longest buffer.
 // The first decoder here walked that chain one sequence at a time with every match source read coming back from
-// L2: ~1200 cycles per sequence, 130 ms for a 1.6 MB column of doubles (profiles/r01_lz4.txt).  This one shortens
+// L2: ~1200 cycles per sequence.  This one shortens
 // the chain instead of adding warps:
 //   * phase A: all lanes parse the token stream redundantly (warp-uniform loads) and lane i keeps sequence i of a
 //     group of up to 32 -- the chain per sequence is one cached byte load, the copies are no longer part of it;
@@ -120,7 +120,7 @@ int decompress_envelope_host(const uint8_t* buf, int64_t len, std::vector<uint8_
 //     the input is staged in a small shared-memory ring (coalesced 16-byte loads) and a short sequence -- at most
 //     one length-extension byte each -- is parsed without per-field bounds checks (only the offset is validated);
 //     anything else takes the fully checked path that reads HBM.  (The first version of this kernel spent ~110
-//     instructions per sequence in the parse, 9/10 of its time: profiles/r01_lz4.txt.)
+//     instructions per sequence in the parse, most of its time.)
 // Positions below are "shifted": P = output offset + (dst & 15), so that dst_al = dst - (dst & 15) is 16-byte
 // aligned, byte P lives at dst_al[P] and in ring slot P & (CFG::WIN - 1), and ring vectors line up with HBM vectors.
 constexpr int LZ_MAX_LIT = 32;         // longer literal runs / matches are copied by the whole warp
@@ -144,7 +144,7 @@ struct LzCfg {
   static_assert(2 * PIECE_ + LZ_GROUP_OUT + 16 <= WIN_ && 2 * LZ_GROUP_OUT + 16 <= WIN_, "output ring too small");
   static_assert(LZ_GROUP_IN + 512 <= IN_, "input ring too small");
 };
-// The default is the shape every measurement and sanitizer run of round 1 was taken with (profiles/r01_lz4.txt).
+// LzDefault is the original shape (4 warps per CTA).
 // LzDense trades ring size for residency: the launch is a latency chain per buffer, so the aggregate expansion rate is
 // (resident buffers) x (bytes per chain-time); with 1 warp and 10 KB per CTA 20 buffers fit an SM instead of 8.  It is
 // selected with SD_TUNE_LZ4_DENSE=1; it passes the GPU parity tests (byte-exact against liblz4) but has not been TIMED
@@ -498,8 +498,8 @@ int lz4_launch_shape(cudaStream_t stream, const Lz4Job* d_jobs, int njobs, unsig
 }
 
 int lz4_launch(cudaStream_t stream, const Lz4Job* d_jobs, int njobs, unsigned int* d_error) {
-  // defaults (profiles/r02_lz4.txt): the dense shape (1 warp + ~11 KB of shared memory per CTA: ~19 buffers resident per SM)
-  // with the window parse: 127 GB/s of expanded output at 6000 buffers vs 45 GB/s for the round-1 default
+  // defaults: the dense shape (1 warp + ~11 KB of shared memory per CTA: ~19 buffers resident per SM) with the window
+  // parse, which expand far more bytes per second with the GPU full of buffers than LzDefault with the serial parse
   static const bool dense = getenv("SD_TUNE_LZ4_DENSE") == nullptr || atoi(getenv("SD_TUNE_LZ4_DENSE")) > 0;
   static const bool wparse = getenv("SD_TUNE_LZ4_PARSE") == nullptr || atoi(getenv("SD_TUNE_LZ4_PARSE")) > 0;
   return lz4_launch_shape(stream, d_jobs, njobs, d_error, dense, wparse);

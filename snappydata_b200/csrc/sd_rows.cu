@@ -2,8 +2,8 @@
 //
 // The scan kernel leaves one fixed-width record per passing row ([batch ordinal | null bits][8 bytes per projected field], string
 // fields as dictionary codes or positions of the value's [len][bytes] record).  Round 1 / early round 2 read the records back
-// and built the rows in a host loop: ~80 ns per row (dictionary lookups that miss the cache, a serial writer) -- 82 ms of a
-// 134 ms C4 step for 1 M rows (profiles/r02_c4_host_laps.txt).  Here the rows are sized, laid out (exclusive scan) and written
+// and built the rows in a host loop (dictionary lookups that miss the cache, a serial writer), which took most of a C4
+// step.  Here the rows are sized, laid out (exclusive scan) and written
 // by the GPU, where the dictionaries already are, and leave in ONE copy straight into the caller's buffer.
 //
 // Row format (what ColumnTableScan's generated code appends to its output buffer, and what
@@ -172,7 +172,10 @@ int device_write_rows(cudaStream_t st, const uint64_t* d_recs, int64_t count, in
   if (!b.d_err) RW(cudaMalloc(reinterpret_cast<void**>(&b.d_err), 8));
   RW(cudaMemsetAsync(b.d_err, 0, 8, st));
   P.offs = b.d_offs; P.err = b.d_err;
-  const int blocks = (int)std::min<int64_t>(148 * 8, (count + 256) / 256);
+  int dev = 0, sms = 0;
+  RW(cudaGetDevice(&dev));
+  RW(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int blocks = (int)std::min<int64_t>(sms * 8, (count + 256) / 256);
   row_sizes_kernel<<<blocks, 256, 0, st>>>(P);
   RW(cudaGetLastError());
   size_t tmp = 0;
@@ -189,7 +192,7 @@ int device_write_rows(cudaStream_t st, const uint64_t* d_recs, int64_t count, in
   if (rc) return rc;
   RW(cudaMemsetAsync(b.d_rows, 0, (size_t)total, st));
   P.out = b.d_rows;
-  const int wblocks = (int)std::min<int64_t>(148 * 8, (count * 32 + 255) / 256);
+  const int wblocks = (int)std::min<int64_t>(sms * 8, (count * 32 + 255) / 256);
   row_write_kernel<<<wblocks, 256, 0, st>>>(P);
   RW(cudaGetLastError());
   *total_out = total;

@@ -570,7 +570,7 @@ int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals) {
   sb->num_rows = b->num_rows; sb->bucket_id = b->bucket_id; sb->batch_id = b->batch_id;
   sb->cols.resize(s->schema.size());
   {   // LZ4 envelopes that lie (almost) back to back in host memory: one host->device copy for the lot (small copies reach
-      // ~42 GB/s on this link, large ones ~54: profiles/r02_lz4.txt)
+      // a lower link rate than large ones)
     s->span_h0 = nullptr;
     const uint8_t *lo = nullptr, *hi = nullptr;
     size_t sum = 0;

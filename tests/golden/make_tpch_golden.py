@@ -1,8 +1,9 @@
-"""Builds tests/golden/tpch_lineitem.npz from the reference's own TPC-H fixture (run in the build
-container only; /root/reference does not exist on the GPU box):
+"""Builds tests/golden/tpch_lineitem.npz from the reference's own TPC-H fixture.  The tests read only the
+stored .npz; this script needs a SnappyData source checkout, given as its argument:
 
-  input   /root/reference/tests/common/src/main/resources/TPCH/lineitem.tbl        (30,201 rows)
-  golden  /root/reference/tests/common/src/main/resources/TPCH/RESULT/Snappy_1.out, Snappy_6.out
+  usage   python tests/golden/make_tpch_golden.py SNAPPYDATA_CHECKOUT
+  input   SNAPPYDATA_CHECKOUT/tests/common/src/main/resources/TPCH/lineitem.tbl        (30,201 rows)
+  golden  SNAPPYDATA_CHECKOUT/tests/common/src/main/resources/TPCH/RESULT/Snappy_1.out, Snappy_6.out
           (the expected lines TPCHDUnitTest compares against,
            cluster/src/dunit/scala/org/apache/spark/sql/TPCHDUnitTest.scala:643-700)
 
@@ -21,11 +22,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 from snappydata_b200.column_format import SqlType, build_batch  # noqa: E402
 
-REF = "/root/reference/tests/common/src/main/resources/TPCH"
+TPCH = os.path.join("tests", "common", "src", "main", "resources", "TPCH")
 EPOCH = datetime.date(1970, 1, 1)
 
 
-def main():
+def main(checkout):
+    REF = os.path.join(checkout, TPCH)
     rows = [l.rstrip("\n").split("|") for l in open(os.path.join(REF, "lineitem.tbl"))]
     n = len(rows)
     orderkey = np.array([int(r[0]) for r in rows])
@@ -64,4 +66,6 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    if len(sys.argv) != 2:
+        sys.exit(__doc__)
+    main(sys.argv[1])

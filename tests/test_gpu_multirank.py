@@ -1,6 +1,6 @@
 """N > 1 on hardware: the NCCL exchange behind the C ABI (sd_comm_* / sd_plan_exchange) under the driver's own launch
-(torchrun, one rank per GPU).  Needs >= 2 GPUs: skipped on a single-GPU box (bench.py's parity_check covers N > 1 there
-whenever the bench itself is run on several GPUs; profiles/r02_multirank.txt holds a run of this test on 2 B200s)."""
+(torchrun, one rank per GPU).  Needs >= 2 GPUs: skipped on a single-GPU machine (bench.py's parity_check covers N > 1
+whenever the bench itself is run on several GPUs)."""
 import os
 import subprocess
 import sys

@@ -14,7 +14,7 @@ def main():
     src = ('#include "sd_kernels.cuh"\n' + g["source"]).encode()
     err, prog = nvrtc.nvrtcCreateProgram(src, b"plan.cu", 2, hdrs, [b"sd_device.h", b"sd_kernels.cuh"])
     nvrtc.nvrtcAddNameExpression(prog, ("sd::scan_aggregate_kernel<%s>" % g["name"]).encode())
-    opts = [b"--gpu-architecture=sm_100a", b"-std=c++17", b"--fmad=false", b"-default-device"] + [e.encode() for e in extra]
+    opts = [b"--gpu-architecture=sm_90a", b"-std=c++17", b"--fmad=false", b"-default-device"] + [e.encode() for e in extra]
     t = time.time()
     (err,) = nvrtc.nvrtcCompileProgram(prog, len(opts), opts)
     dt = time.time() - t

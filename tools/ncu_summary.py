@@ -1,6 +1,6 @@
 """Per-launch summary of an `ncu -i X.ncu-rep --page raw --csv` dump: the metrics the DESIGN / judge read (duration, DRAM bytes
 and throughput, shared-memory pipe, issue slots, occupancy limits, registers, stall reasons).
-usage: python tools/ncu_summary.py raw.csv > profiles/rNN_xxx.txt"""
+usage: python tools/ncu_summary.py raw.csv > summary.txt"""
 import csv
 import sys
 
