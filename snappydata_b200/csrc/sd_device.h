@@ -49,6 +49,7 @@ constexpr int MAX_RPT = 8;
 // bytes one row of a column occupies in a stage of the shared-memory ring (K_CODE: room for int32 indexes)
 constexpr int kind_stage_width(int k) { return (k == K_I64 || k == K_F64) ? 8 : (k == K_I32 || k == K_F32 || k == K_CODE) ? 4 : (k == K_I16) ? 2 : 1; }
 constexpr int MAX_STAGES = 12;
+constexpr int RING_ALIGN_SLACK = 128;   // shared memory reserved to start the ring on a 128-byte boundary (sd_kernels.cuh)
 
 // bytes of TileSmem<PLAN> for a plan with nc scan columns (kept in sync with sd_kernels.cuh)
 constexpr int tile_smem_bytes(int nc, int rpt) {

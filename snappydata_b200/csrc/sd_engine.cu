@@ -809,7 +809,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
     }
   }
   const size_t tile_smem = k->tile_smem;
-  const size_t ring_fixed = 2 * MAX_STAGES * 8;
+  const size_t ring_fixed = 2 * MAX_STAGES * 8 + RING_ALIGN_SLACK;   // mbarriers + alignment of the ring
   const size_t min_ring = k->staged ? ring_fixed + 2 * k->stage_bytes + 128 : 0;
   size_t table_bytes = (size_t)std::max(ns, 1) * (THREADS / 32) * 8;
   if (sp.mode == MODE_GROUPS && table_mode != TABLE_REGS) {

@@ -1002,9 +1002,12 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   const DevBatch<PLAN::NC>* batches = reinterpret_cast<const DevBatch<PLAN::NC>*>(args.batches);
 
   // ---- staged fast path: [full barriers][empty barriers][ring of nstages stages] -----------------------
+  // The ring starts on a 128-byte boundary of the shared window, so that every bulk copy lands 128-byte aligned (each
+  // column region of a stage is a multiple of 128 bytes).  Dynamic shared memory itself starts behind the kernel's static
+  // shared variables, at an address that is only 16-byte aligned: the engine reserves RING_ALIGN_SLACK bytes for this.
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_raw + args.ring_off);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint8_t* ring = smem_raw + args.ring_off + 2 * MAX_STAGES * 8;
+  uint8_t* ring = smem_raw + ((smem_u32(smem_raw) + args.ring_off + 2 * MAX_STAGES * 8 + 127) & ~127u) - smem_u32(smem_raw);
   const int nstages = args.nstages;
   if (PLAN::STAGES > 0) {
     if (tid == 0) {
