@@ -313,6 +313,10 @@ int sdx_decompress_envelope(const void* buf, int64_t len, void* out, int64_t cap
 int sdx_store_get_stats(sd_store* s, int64_t batch_index, void* out, int64_t cap, int64_t* out_len);
 int sdx_store_batch_info(sd_store* s, int64_t batch_index, int32_t* num_rows, int32_t* bucket_id,
                          int64_t* batch_id);
+/* device memory held by a store: the bytes of its slabs, and how many of them the driver allocated as compressible (the
+ * store asks for generic compression where the device reports support; the hardware then compresses those slabs between
+ * L2 and DRAM, invisibly to kernels and copies).  Read only. */
+int sdx_store_memory_info(sd_store* s, int64_t* compressible_bytes, int64_t* slab_bytes);
 /* the batch-skipping decision (ColumnTableScan.scala:820-963) of a plan's filter for one stats row: *pass = 0 when the
  * batch would be skipped.  Host only, no CUDA call (test hook: tests/test_stats_predicate.py compares it with the oracle). */
 int sdx_stats_pass(const sd_plan_desc* desc, const sd_literal* lits, int32_t nlits, const void* stats,

@@ -253,6 +253,8 @@ def product_api() -> Api:
         L.sdx_store_get_buffer.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
         L.sdx_store_batch_info.restype = C.c_int
         L.sdx_store_batch_info.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
+        L.sdx_store_memory_info.restype = C.c_int
+        L.sdx_store_memory_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     return _product
 
 
@@ -641,6 +643,12 @@ class Store:
         n, b, i = C.c_int32(), C.c_int32(), C.c_int64()
         self.api.check(self.api.lib.sdx_store_batch_info(self.h, batch_index, C.byref(n), C.byref(b), C.byref(i)))
         return n.value, b.value, i.value
+
+    def memory_info(self):
+        """(compressible bytes, slab bytes) of the device memory the store holds."""
+        comp, total = C.c_int64(), C.c_int64()
+        self.api.check(self.api.lib.sdx_store_memory_info(self.h, C.byref(comp), C.byref(total)))
+        return comp.value, total.value
 
     def close(self):
         if self.h:

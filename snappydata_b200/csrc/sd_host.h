@@ -99,7 +99,18 @@ int comm_all_gather_bytes(void* c, const void* d_send, void* d_recv, size_t byte
 struct Arena {
   int device = 0;
   size_t slab_bytes = size_t(512) << 20;
-  std::vector<std::pair<uint8_t*, size_t>> slabs;
+  // slabs from cuMemCreate with generic compression requested, where the device reports support for it: the hardware
+  // compresses them between L2 and DRAM, so a scan of compressible bytes moves fewer DRAM bytes; what kernels and copies
+  // see is unchanged.  Set for the resident store only; everything else stays on cudaMalloc.
+  bool compressible = false;
+  struct Slab {
+    uint8_t* base;
+    size_t bytes;
+    bool vmm;                   // cuMemCreate + cuMemMap (else cudaMalloc)
+    bool compressed;            // the driver granted generic compression
+    unsigned long long handle;  // CUmemGenericAllocationHandle of a vmm slab
+  };
+  std::vector<Slab> slabs;
   size_t cur_slab = 0;
   size_t cur_off = 0;
   size_t used = 0;

@@ -7,6 +7,9 @@
 // by the engine: every buffer is positioned so that its first value / first dictionary index is
 // 128-byte aligned, which makes every vector load of the scan kernel naturally aligned.  Null words get
 // an 8-byte aligned side copy plus a host-computed "nulls before" prefix (one int32 per 512 rows).
+#include <cuda.h>
+#include <cudaTypedefs.h>
+
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -47,16 +50,106 @@ AotRegistrar::AotRegistrar(const char* signature, const void* func, size_t tile_
 }
 
 // ---- arena ------------------------------------------------------------------------------------------
+// the driver's virtual memory calls, resolved through the runtime (the library does not link libcuda)
+namespace {
+struct Vmm {
+  PFN_cuDeviceGet_v2000 device_get = nullptr;
+  PFN_cuDeviceGetAttribute_v2000 attribute = nullptr;
+  PFN_cuMemGetAllocationGranularity_v10020 granularity = nullptr;
+  PFN_cuMemCreate_v10020 create = nullptr;
+  PFN_cuMemGetAllocationPropertiesFromHandle_v10020 props = nullptr;
+  PFN_cuMemAddressReserve_v10020 reserve = nullptr;
+  PFN_cuMemMap_v10020 map = nullptr;
+  PFN_cuMemSetAccess_v10020 set_access = nullptr;
+  PFN_cuMemUnmap_v10020 unmap = nullptr;
+  PFN_cuMemRelease_v10020 release = nullptr;
+  PFN_cuMemAddressFree_v10020 address_free = nullptr;
+  bool ok = false;
+};
+const Vmm& vmm() {
+  static const Vmm v = [] {
+    Vmm t;
+    auto get = [](const char* name, void** fn) {
+      cudaDriverEntryPointQueryResult q;
+      return cudaGetDriverEntryPointByVersion(name, fn, 12000, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess;
+    };
+    t.ok = get("cuDeviceGet", (void**)&t.device_get) && get("cuDeviceGetAttribute", (void**)&t.attribute) &&
+           get("cuMemGetAllocationGranularity", (void**)&t.granularity) && get("cuMemCreate", (void**)&t.create) &&
+           get("cuMemGetAllocationPropertiesFromHandle", (void**)&t.props) && get("cuMemAddressReserve", (void**)&t.reserve) &&
+           get("cuMemMap", (void**)&t.map) && get("cuMemSetAccess", (void**)&t.set_access) && get("cuMemUnmap", (void**)&t.unmap) &&
+           get("cuMemRelease", (void**)&t.release) && get("cuMemAddressFree", (void**)&t.address_free);
+    return t;
+  }();
+  return v;
+}
+#define SD_CU(call, what)                                                                        \
+  do {                                                                                         \
+    CUresult r__ = (call);                                                                     \
+    if (r__ != CUDA_SUCCESS) { set_error(SD_ERR_CUDA, "%s failed: CUresult %d", what, (int)r__); goto fail; } \
+  } while (0)
+
+// 1: the device compresses generic allocations (*gran: their granularity); 0: it does not; < 0: error set
+int compression_granularity(int device, size_t* gran) {
+  const Vmm& v = vmm();
+  if (!v.ok) return set_error(SD_ERR_CUDA, "the CUDA driver lacks the virtual memory entry points");
+  CUdevice dev;
+  int supported = 0;
+  CUmemAllocationProp prop = {};
+  if (v.device_get(&dev, device) != CUDA_SUCCESS ||
+      v.attribute(&supported, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, dev) != CUDA_SUCCESS)
+    return set_error(SD_ERR_CUDA, "device %d: compression support query failed", device);
+  if (!supported) return 0;
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = dev;
+  prop.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+  if (v.granularity(gran, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED) != CUDA_SUCCESS)
+    return set_error(SD_ERR_CUDA, "device %d: compressible allocation granularity query failed", device);
+  return 1;
+}
+
+// a compressible slab of at least `want` bytes; false: error set, nothing held
+bool vmm_slab(int device, size_t want, size_t gran, Arena::Slab* out) {
+  const Vmm& v = vmm();
+  const size_t sz = (want + gran - 1) / gran * gran;
+  CUmemAllocationProp prop = {}, got = {};
+  CUmemGenericAllocationHandle h = 0;
+  CUdeviceptr va = 0;
+  CUmemAccessDesc access = {};
+  bool created = false, mapped = false;
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  prop.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+  SD_CU(v.create(&h, sz, &prop, 0), "cuMemCreate");
+  created = true;
+  SD_CU(v.props(&got, h), "cuMemGetAllocationPropertiesFromHandle");
+  SD_CU(v.reserve(&va, sz, gran, 0, 0), "cuMemAddressReserve");
+  SD_CU(v.map(va, sz, 0, h, 0), "cuMemMap");
+  mapped = true;
+  access.location = prop.location;
+  access.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  SD_CU(v.set_access(va, sz, &access, 1), "cuMemSetAccess");
+  *out = {reinterpret_cast<uint8_t*>(va), sz, true, got.allocFlags.compressionType == CU_MEM_ALLOCATION_COMP_GENERIC, h};
+  return true;
+fail:
+  if (mapped) v.unmap(va, sz);
+  if (va) v.address_free(va, sz);
+  if (created) v.release(h);
+  return false;
+}
+}  // namespace
+
 uint8_t* Arena::alloc(size_t n, size_t align, size_t misalign) {
   if (n == 0) n = 1;
   for (;;) {
     if (cur_slab < slabs.size()) {
-      uint8_t* base = slabs[cur_slab].first;
+      uint8_t* base = slabs[cur_slab].base;
       size_t p = (size_t)(uintptr_t)(base + cur_off);
       size_t want = (p + misalign + align - 1) / align * align - misalign;
       if (want < p) want += align;
       size_t off = want - (size_t)(uintptr_t)base;
-      if (off + n <= slabs[cur_slab].second) {
+      if (off + n <= slabs[cur_slab].bytes) {
         cur_off = off + n;
         used += n;
         return base + off;
@@ -67,14 +160,23 @@ uint8_t* Arena::alloc(size_t n, size_t align, size_t misalign) {
     }
     size_t sz = slab_bytes;
     if (n + align + misalign + 256 > sz) sz = n + align + misalign + 256;
-    void* p = nullptr;
     cudaSetDevice(device);
-    cudaError_t e = cudaMalloc(&p, sz);
-    if (e != cudaSuccess) {
-      set_error(SD_ERR_CUDA, "cudaMalloc(%zu) failed: %s", sz, cudaGetErrorString(e));
-      return nullptr;
+    size_t gran = 0;
+    const int comp = compressible ? compression_granularity(device, &gran) : 0;
+    if (comp < 0) return nullptr;
+    if (comp) {
+      Slab sl;
+      if (!vmm_slab(device, sz, gran, &sl)) return nullptr;
+      slabs.push_back(sl);
+    } else {
+      void* p = nullptr;
+      cudaError_t e = cudaMalloc(&p, sz);
+      if (e != cudaSuccess) {
+        set_error(SD_ERR_CUDA, "cudaMalloc(%zu) failed: %s", sz, cudaGetErrorString(e));
+        return nullptr;
+      }
+      slabs.push_back({(uint8_t*)p, sz, false, false, 0});
     }
-    slabs.push_back({(uint8_t*)p, sz});
     cur_slab = slabs.size() - 1;
     cur_off = 0;
   }
@@ -82,7 +184,17 @@ uint8_t* Arena::alloc(size_t n, size_t align, size_t misalign) {
 void Arena::reset() { cur_slab = 0; cur_off = 0; used = 0; }
 void Arena::release() {
   if (!slabs.empty()) cudaSetDevice(device);
-  for (auto& s : slabs) cudaFree(s.first);
+  for (auto& s : slabs) {
+    if (s.vmm) {
+      const Vmm& v = vmm();
+      const CUdeviceptr va = reinterpret_cast<CUdeviceptr>(s.base);
+      v.unmap(va, s.bytes);
+      v.release(s.handle);
+      v.address_free(va, s.bytes);
+    } else {
+      cudaFree(s.base);
+    }
+  }
   slabs.clear();
   reset();
 }
@@ -732,6 +844,7 @@ int sd_store_create(int device, int32_t ncols, const sd_column* schema, sd_store
   sd_store* s = new sd_store();
   s->device = device;
   s->arena.device = device;
+  s->arena.compressible = true;
   s->lz4_stage.device = device;
   s->lz4_stage.slab_bytes = size_t(256) << 20;
   s->schema.assign(schema, schema + ncols);
@@ -756,6 +869,17 @@ int sd_store_put_batch(sd_store* s, const sd_batch* b) {
 
 int sd_store_num_batches(sd_store* s, int64_t* out) { std::lock_guard<std::mutex> lock(s->mu); *out = (int64_t)s->batches.size(); return 0; }
 int sd_store_bytes(sd_store* s, int64_t* out) { std::lock_guard<std::mutex> lock(s->mu); *out = (int64_t)s->arena.used; return 0; }
+int sdx_store_memory_info(sd_store* s, int64_t* compressible_bytes, int64_t* slab_bytes) {
+  if (!s || !compressible_bytes || !slab_bytes) return sd::set_error(SD_ERR_INVALID, "sdx_store_memory_info: null argument");
+  std::lock_guard<std::mutex> lock(s->mu);
+  *compressible_bytes = 0;
+  *slab_bytes = 0;
+  for (const auto& sl : s->arena.slabs) {
+    *slab_bytes += (int64_t)sl.bytes;
+    if (sl.compressed) *compressible_bytes += (int64_t)sl.bytes;
+  }
+  return 0;
+}
 
 void sd_store_destroy(sd_store* s) {
   if (!s) return;

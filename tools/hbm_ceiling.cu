@@ -13,8 +13,22 @@
 //           consumers only release stages (what is left for the consumers' work)
 //   r3lds   r3, and the consumers also read their rows of every column out of the stage (the scan's LDS, no arithmetic)
 //
+// Two more dimensions say whether Hopper's generic memory compression (done by the hardware between L2 and DRAM, invisible
+// to kernels) lowers the DRAM bytes behind those reads:
+//   --alloc plain          one cudaMalloc (never compressible)
+//   --alloc compressible   512 MB chunks from cuMemCreate with allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC,
+//                          mapped back to back into one reserved range; what the driver granted is read back per chunk
+//   --fill const           every byte 0x5a (the positive control: the most compressible content there is)
+//   --fill random          splitmix64 bytes (the negative control)
+//   --fill q1              every column stream holds the lineitem generator's values (snappydata_b200/lineitem.py; the
+//                          dictionary codes are the flag classes, the same {0,1,2} value set the store's codes take)
+//   --fill q1:<column>     only that column holds generator values, the others random bytes (which columns compress)
+//
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o hbm_ceiling hbm_ceiling.cu
-// usage: hbm_ceiling <r1|r2|r3|r3lds> [--ctas-per-sm N] [--stages N] [--reps N] [--warmup N]
+// usage: hbm_ceiling <r1|r2|r3|r3lds> [--ctas-per-sm N] [--stages N] [--reps N] [--warmup N] [--alloc plain|compressible]
+//                    [--fill const|random|q1|q1:<column>]
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cstdint>
@@ -25,6 +39,7 @@
 #include <vector>
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { fprintf(stderr, "%s:%d %s: %s\n", __FILE__, __LINE__, #x, cudaGetErrorString(e_)); exit(1); } } while (0)
+#define CU(x) do { CUresult r_ = (x); if (r_ != CUDA_SUCCESS) { fprintf(stderr, "%s:%d %s: CUresult %d\n", __FILE__, __LINE__, #x, (int)r_); exit(1); } } while (0)
 
 constexpr int64_t ROWS = 600037902;      // TPC-H SF-100 lineitem
 constexpr int ROWS_PER_BATCH = 200000;   // bench.py's batch size
@@ -41,6 +56,43 @@ __device__ __forceinline__ uint32_t fold(uint4 v) { return v.x ^ v.y ^ v.z ^ v.w
 __device__ __forceinline__ void publish(uint32_t x, unsigned* out) {
   for (int d = 16; d > 0; d >>= 1) x ^= __shfl_xor_sync(0xffffffffu, x, d);
   if ((threadIdx.x & 31) == 0) atomicXor(out, x);
+}
+
+// ---- fills --------------------------------------------------------------------------------------------
+__host__ __device__ inline uint64_t mix64(uint64_t x) {
+  x += 0x9E3779B97F4A7C15ull;
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+__device__ inline uint64_t hrow(uint64_t row, int stream, uint64_t seed) { return mix64(seed ^ mix64(row * 16 + (uint64_t)stream)); }
+
+__global__ void random_fill_kernel(uint64_t* p, int64_t n8) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) p[i] = mix64(~(uint64_t)i);
+}
+
+// column c of every row: the generator's value where bit c of `mask` is set, random bytes elsewhere
+__global__ void q1_fill_kernel(const Batch* batches, int mask, uint64_t seed) {
+  for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < ROWS; row += (int64_t)gridDim.x * blockDim.x) {
+    const Batch& b = batches[row / ROWS_PER_BATCH];
+    const int64_t i = row % ROWS_PER_BATCH;
+    const uint64_t r = (uint64_t)row;
+    const int32_t ship = 8036 + (int32_t)(hrow(r, 4, seed) % 2526ull);
+    const int fr = (int)(hrow(r, 5, seed) % 100ull);
+    const int16_t rf = ship > 9298 ? 0 : fr < 2 ? 0 : fr < 51 ? 1 : 2, ls = ship > 9298 ? 0 : 1;
+    const double q = (double)(1ull + hrow(r, 0, seed) % 50ull), pr = (double)(90000ull + hrow(r, 1, seed) % 10410000ull) / 100.0;
+    const double di = (double)(hrow(r, 2, seed) % 11ull) / 100.0, tx = (double)(hrow(r, 3, seed) % 9ull) / 100.0;
+    const double dv[4] = {q, pr, di, tx};
+#pragma unroll
+    for (int c = 0; c < NC; c++) {
+      const uint64_t junk = mix64(~(r * NC + c));
+      uint8_t* dst = const_cast<uint8_t*>(b.data[c]) + i * width(c);
+      const bool gen = (mask >> c) & 1;
+      if (width(c) == 8) *reinterpret_cast<uint64_t*>(dst) = gen ? (uint64_t)__double_as_longlong(dv[c < 4 ? c : 0]) : junk;
+      else if (width(c) == 4) *reinterpret_cast<int32_t*>(dst) = gen ? ship : (int32_t)junk;
+      else *reinterpret_cast<int16_t*>(dst) = gen ? (c == 4 ? rf : ls) : (int16_t)junk;
+    }
+  }
 }
 
 // ---- r1 -------------------------------------------------------------------------------------------
@@ -197,10 +249,46 @@ __global__ void __launch_bounds__(THREADS + 32, 1) r3_kernel(const Batch* batche
 }
 
 // ---- host ----------------------------------------------------------------------------------------------
+static const char* const COLUMN_NAMES[NC] = {"quantity", "extendedprice", "discount", "tax", "returnflag", "linestatus", "shipdate"};
+
+// compressible memory: the driver entry points through the runtime, so the probe needs no -lcuda
+struct Vmm {
+  PFN_cuMemCreate_v10020 create;
+  PFN_cuMemRelease_v10020 release;
+  PFN_cuMemAddressReserve_v10020 reserve;
+  PFN_cuMemAddressFree_v10020 free_range;
+  PFN_cuMemMap_v10020 map;
+  PFN_cuMemUnmap_v10020 unmap;
+  PFN_cuMemSetAccess_v10020 set_access;
+  PFN_cuMemGetAllocationGranularity_v10020 granularity;
+  PFN_cuMemGetAllocationPropertiesFromHandle_v10020 props;
+  PFN_cuDeviceGetAttribute_v2000 attribute;
+  void load() {
+    auto get = [](const char* name, void** fn) {
+      cudaDriverEntryPointQueryResult q;
+      CK(cudaGetDriverEntryPointByVersion(name, fn, 12000, cudaEnableDefault, &q));
+      if (q != cudaDriverEntryPointSuccess) { fprintf(stderr, "driver entry point %s not found\n", name); exit(1); }
+    };
+    get("cuMemCreate", (void**)&create);
+    get("cuMemRelease", (void**)&release);
+    get("cuMemAddressReserve", (void**)&reserve);
+    get("cuMemAddressFree", (void**)&free_range);
+    get("cuMemMap", (void**)&map);
+    get("cuMemUnmap", (void**)&unmap);
+    get("cuMemSetAccess", (void**)&set_access);
+    get("cuMemGetAllocationGranularity", (void**)&granularity);
+    get("cuMemGetAllocationPropertiesFromHandle", (void**)&props);
+    get("cuDeviceGetAttribute", (void**)&attribute);
+  }
+};
+
 int main(int argc, char** argv) {
-  if (argc < 2) { fprintf(stderr, "usage: %s <r1|r2|r3|r3lds> [--ctas-per-sm N] [--stages N] [--reps N] [--warmup N]\n", argv[0]); return 2; }
+  const char* usage = "usage: %s <r1|r2|r3|r3lds> [--ctas-per-sm N] [--stages N] [--reps N] [--warmup N] [--alloc plain|compressible] "
+                      "[--fill const|random|q1|q1:<column>]\n";
+  if (argc < 2) { fprintf(stderr, usage, argv[0]); return 2; }
   const std::string variant = argv[1];
   int ctas_per_sm = variant == "r1" ? 4 : variant == "r2" ? 4 : 1, nstages = 3, reps = 30, warmup = 60;
+  std::string alloc = "plain", fill = "const";
   for (int i = 2; i + 1 < argc; i += 2) {
     const std::string k = argv[i];
     const int v = atoi(argv[i + 1]);
@@ -208,14 +296,24 @@ int main(int argc, char** argv) {
     else if (k == "--stages") nstages = v;
     else if (k == "--reps") reps = v;
     else if (k == "--warmup") warmup = v;
+    else if (k == "--alloc") alloc = argv[i + 1];
+    else if (k == "--fill") fill = argv[i + 1];
     else { fprintf(stderr, "unknown option %s\n", k.c_str()); return 2; }
   }
   if (variant != "r1" && variant != "r2" && variant != "r3" && variant != "r3lds") { fprintf(stderr, "unknown variant %s\n", variant.c_str()); return 2; }
   if (nstages < 2 || nstages > MAX_STAGES || reps < 1) { fprintf(stderr, "bad --stages / --reps\n"); return 2; }
+  if (alloc != "plain" && alloc != "compressible") { fprintf(stderr, "unknown --alloc %s\n", alloc.c_str()); return 2; }
+  int q1_mask = -1;   // -1: not a q1 fill
+  if (fill == "q1") q1_mask = (1 << NC) - 1;
+  else if (fill.rfind("q1:", 0) == 0) {
+    for (int c = 0; c < NC; c++) if (fill.substr(3) == COLUMN_NAMES[c]) q1_mask = 1 << c;
+    if (q1_mask < 0) { fprintf(stderr, "unknown column in --fill %s\n", fill.c_str()); return 2; }
+  } else if (fill != "const" && fill != "random") { fprintf(stderr, "unknown --fill %s\n", fill.c_str()); return 2; }
 
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, 0));
   const int sms = prop.multiProcessorCount;
+  CK(cudaFree(nullptr));   // create the context before any driver call
 
   // placement: every column buffer of a batch bump-allocated in 512 MB slabs, value start 128-byte aligned, 160 bytes of
   // tail padding; r1 reads the first `algo` bytes of the same allocation contiguously
@@ -238,10 +336,44 @@ int main(int argc, char** argv) {
       algo += (int64_t)rows * width(c);
     }
   }
-  const size_t span = slab_base + off + 4096;
+  size_t span = slab_base + off + 4096;
   uint8_t* d = nullptr;
-  CK(cudaMalloc(&d, span));
-  CK(cudaMemset(d, 0x5a, span));
+  int comp_supported = -1, chunks = 0, chunks_compressed = 0;
+  size_t gran = 0, chunk_bytes = 0;
+  Vmm vmm{};
+  std::vector<CUmemGenericAllocationHandle> handles;
+  CUdeviceptr range = 0;
+  if (alloc == "plain") {
+    CK(cudaMalloc(&d, span));
+  } else {
+    vmm.load();
+    CUdevice dev = 0;
+    CU(vmm.attribute(&comp_supported, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, dev));
+    CUmemAllocationProp ap = {};
+    ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    ap.location.id = dev;
+    ap.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+    CU(vmm.granularity(&gran, &ap, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED));
+    chunk_bytes = (SLAB + gran - 1) / gran * gran;
+    span = (span + chunk_bytes - 1) / chunk_bytes * chunk_bytes;
+    CU(vmm.reserve(&range, span, chunk_bytes, 0, 0));
+    for (size_t o = 0; o < span; o += chunk_bytes) {
+      CUmemGenericAllocationHandle h;
+      CU(vmm.create(&h, chunk_bytes, &ap, 0));
+      CUmemAllocationProp got = {};
+      CU(vmm.props(&got, h));
+      chunks++;
+      chunks_compressed += got.allocFlags.compressionType == CU_MEM_ALLOCATION_COMP_GENERIC;
+      CU(vmm.map(range + o, chunk_bytes, 0, h, 0));
+      handles.push_back(h);
+    }
+    CUmemAccessDesc acc = {};
+    acc.location = ap.location;
+    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+    CU(vmm.set_access(range, span, &acc, 1));
+    d = reinterpret_cast<uint8_t*>(range);
+  }
   for (int b = 0; b < nb; b++)
     for (int c = 0; c < NC; c++) hb[b].data[c] = d + offs[(size_t)b * NC + c];
   Batch* d_batches = nullptr;
@@ -253,6 +385,14 @@ int main(int argc, char** argv) {
   CK(cudaMemcpy(d_batches, hb.data(), sizeof(Batch) * nb, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_prefix, prefix.data(), sizeof(int32_t) * (nb + 1), cudaMemcpyHostToDevice));
   CK(cudaMemset(d_out, 0, sizeof(unsigned)));
+  if (fill == "const") CK(cudaMemset(d, 0x5a, span));
+  else if (fill == "random") random_fill_kernel<<<sms * 8, 256>>>(reinterpret_cast<uint64_t*>(d), (int64_t)(span / 8));
+  else {
+    CK(cudaMemset(d, 0, span));   // headers, alignment gaps and tail padding stay zero, as an arena slab's unwritten bytes
+    q1_fill_kernel<<<sms * 8, 256>>>(d_batches, q1_mask, 1);
+  }
+  CK(cudaGetLastError());
+  CK(cudaDeviceSynchronize());
   const int items = prefix[nb];
 
   size_t smem = 0;
@@ -287,13 +427,20 @@ int main(int argc, char** argv) {
   unsigned h_out = 0;
   CK(cudaMemcpy(&h_out, d_out, sizeof(unsigned), cudaMemcpyDeviceToHost));
   const double med = ms[reps / 2], best = ms[0];
-  printf("{\"variant\": \"%s\", \"grid\": %d, \"threads\": %d, \"stages\": %d, \"stage_bytes\": %d, \"smem\": %zu, \"bytes\": %lld, "
+  printf("{\"alloc\": \"%s\", \"fill\": \"%s\", \"compression_supported\": %d, \"granularity\": %zu, \"chunk_bytes\": %zu, "
+         "\"chunks\": %d, \"chunks_compressed\": %d, ", alloc.c_str(), fill.c_str(), comp_supported, gran, chunk_bytes, chunks, chunks_compressed);
+  printf("\"variant\": \"%s\", \"grid\": %d, \"threads\": %d, \"stages\": %d, \"stage_bytes\": %d, \"smem\": %zu, \"bytes\": %lld, "
          "\"reps\": %d, \"ms_median\": %.4f, \"ms_min\": %.4f, \"ms_max\": %.4f, \"gbps_median\": %.1f, \"gbps_best\": %.1f, \"check\": %u}\n",
          variant.c_str(), variant.rfind("r3", 0) == 0 ? sms : grid, variant == "r1" ? 512 : variant == "r2" ? THREADS : THREADS + 32,
          variant.rfind("r3", 0) == 0 ? nstages : 0, STAGE_BYTES, smem, (long long)algo, reps, med, best, ms[reps - 1],
          algo / (med * 1e-3) / 1e9, algo / (best * 1e-3) / 1e9, h_out);
   for (auto& e : ev) cudaEventDestroy(e);
-  cudaFree(d);
+  if (alloc == "plain") cudaFree(d);
+  else {
+    CU(vmm.unmap(range, span));
+    for (auto h : handles) CU(vmm.release(h));
+    CU(vmm.free_range(range, span));
+  }
   cudaFree(d_batches);
   cudaFree(d_prefix);
   cudaFree(d_out);

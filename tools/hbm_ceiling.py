@@ -3,7 +3,10 @@ directory, runs each variant in its own process and samples the SM clock with a 
 beside it (the same query bench.py's ClockSampler makes).  Prints one JSON line per variant and a header line with the
 card's name, power limit and maximum clocks.
 
-    python tools/hbm_ceiling.py [--out FILE] [--reps N]
+    python tools/hbm_ceiling.py [--out FILE] [--reps N] [--allocs plain,compressible] [--fills const,random,q1,q1:shipdate,...]
+
+With --allocs or --fills it runs R1 and R2 (4 CTAs/SM) and R3 (3 stages) for every allocation x fill combination instead of the
+grid and stage sweep below: whether generic memory compression lowers the DRAM bytes behind the scan's reads.
 """
 import argparse
 import json
@@ -22,6 +25,7 @@ RUNS = [("r1", ["--ctas-per-sm", "2"]), ("r1", ["--ctas-per-sm", "4"]),
         ("r2", ["--ctas-per-sm", "2"]), ("r2", ["--ctas-per-sm", "4"]), ("r2", ["--ctas-per-sm", "8"]),
         ("r3", ["--stages", "2"]), ("r3", ["--stages", "3"]), ("r3", ["--stages", "4"]), ("r3", ["--stages", "5"]),
         ("r3lds", ["--stages", "3"]), ("r3lds", ["--stages", "5"])]
+COMPRESSION_RUNS = [("r1", ["--ctas-per-sm", "4"]), ("r2", ["--ctas-per-sm", "4"]), ("r3", ["--stages", "3"])]
 
 CLOCK_Q = "clocks.sm,clocks.mem,power.draw,clocks_event_reasons.sw_power_cap"
 
@@ -69,7 +73,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="also write the lines to this file")
     ap.add_argument("--reps", type=int, default=30)
+    ap.add_argument("--allocs", default=None, help="comma-separated --alloc values")
+    ap.add_argument("--fills", default=None, help="comma-separated --fill values")
     args = ap.parse_args()
+    if args.allocs or args.fills:
+        runs = [(v, opts + ["--alloc", a, "--fill", f]) for a in (args.allocs or "plain").split(",")
+                for f in (args.fills or "const").split(",") for v, opts in COMPRESSION_RUNS]
+    else:
+        runs = RUNS
     lines = []
     with tempfile.TemporaryDirectory() as tmp:
         exe = os.path.join(tmp, "hbm_ceiling")
@@ -78,7 +89,7 @@ def main():
         name, plimit, maxsm, maxmem = smi("name,power.limit,clocks.max.sm,clocks.max.mem")
         lines.append(json.dumps({"gpu": name, "power_limit_w": float(plimit), "sm_max_mhz": float(maxsm), "mem_max_mhz": float(maxmem)}))
         print(lines[-1], flush=True)
-        for variant, opts in RUNS:
+        for variant, opts in runs:
             s = Sampler()
             p = subprocess.run([exe, variant, "--reps", str(args.reps)] + opts, stdout=subprocess.PIPE, text=True)
             clk = s.stop()
