@@ -123,8 +123,12 @@ typedef struct sd_plan_desc {
   int32_t naggs;   const sd_agg* aggs;
   int32_t nproj;   const int32_t* proj;    /* naggs == 0 && nkeys == 0: output columns   */
   int32_t nliterals; const int32_t* literal_types;   /* sd_type per literal slot         */
-  int32_t flags;                /* reserved, 0                                           */
+  int32_t flags;                /* 0, or SD_PLAN_MUTATE                                  */
 } sd_plan_desc;
+
+/* An UPDATE / DELETE over a resident store (sd_plan_update_store / sd_plan_delete_store).  No keys, no aggregates; `filter` is
+ * the WHERE clause (-1: every live row); UPDATE: proj[i] is the value of the i-th SET target; DELETE: nproj = 0. */
+#define SD_PLAN_MUTATE 1
 
 typedef struct sd_literal {
   int32_t type;      /* sd_type                              */
@@ -251,6 +255,23 @@ int sd_store_bytes(sd_store* s, int64_t* out);
 int sd_plan_scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets);
 void sd_store_destroy(sd_store* s);
 
+/* ---- UPDATE / DELETE on the device (the reference's ColumnUpdateExec / ColumnDeleteExec, core/.../columnar/ColumnUpdateExec.scala,
+ *      ColumnDeleteExec.scala, with the store-side merge of ColumnDelta.apply, encoders/.../impl/ColumnDelta.scala:64-222).
+ *      p is an SD_PLAN_MUTATE plan.  The WHERE sees each row's current value (base, depth-1, then depth-0 delta); deleted rows
+ *      are not touched; SET values are computed from the row as it was before the statement.  UPDATE: every touched (batch,
+ *      target) gets a new depth-0 delta = ColumnDeltaEncoder.merge(new, existing depth 0) in the type's default encoding; the
+ *      stats row is merged as ColumnDelta.mergeStats does.  DELETE: the positions are merged into the batch's delete mask; a
+ *      batch whose every row is deleted is no longer scanned.  A statement works on the batches present when it starts; its
+ *      new batch versions are installed together under the store's lock (a scan sees all of them or none); statements on one
+ *      store are serialised; a failing statement installs nothing.  Superseded delta / mask bytes stay in the store's arena
+ *      until the store is destroyed (sd_store_bytes counts them).  Refused: STRING / BOOLEAN targets (SD_ERR_UNSUPPORTED), a SET
+ *      type other than the target's (SD_ERR_INVALID), a target not resident in a touched batch (SD_ERR_INVALID), NULL into a
+ *      NOT NULL target (SD_ERR_INVALID), a plan without SD_PLAN_MUTATE (SD_ERR_STATE). ------------------------------------ */
+int sd_plan_update_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, const sd_literal* lits, int32_t nlits,
+                         const int32_t* target_cols, int64_t* rows_updated);
+int sd_plan_delete_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, const sd_literal* lits, int32_t nlits,
+                         int64_t* rows_deleted);
+
 /* ---- final merge (SnappyHashAggregateExec(Final) / CollectAggregateExec.executeCollect,
  *      core/execution/aggregate/CollectAggregateExec.scala:67-121): merges partial rows of all
  *      partitions (sums add, counts add, min/max combine) and evaluates results (avg = sum/count).
@@ -309,6 +330,16 @@ int64_t sdx_lz4_decode_prefix(const void* src, int64_t src_len, void* dst, int64
 /* host decompression of a stored envelope [-codecId][uncompressedLen][payload] (LZ4 = 1, Snappy = 2), as the engine
  * applies it to update deltas, delete masks and Snappy column buffers (test hook; no CUDA call) */
 int sdx_decompress_envelope(const void* buf, int64_t len, void* out, int64_t cap, int64_t* out_len);
+/* a resident update delta (depth 0 or 1) of a batch's table column in the reference's byte layout (enc/ColumnDeltaEncoder.scala:
+ * 300-331); SD_ERR_INVALID when the column has none at that depth, SD_ERR_UNSUPPORTED for a dictionary / bit-set delta */
+int sdx_store_get_delta(sd_store* s, int64_t batch_index, int32_t table_col, int32_t depth, void* out, int64_t cap,
+                        int64_t* out_len);
+/* the delete mask of a resident batch: [0][numBaseRows][numDeletes][positions] (enc/ColumnDeleteEncoder.scala:101-134);
+ * SD_ERR_INVALID when the batch has none */
+int sdx_store_get_deletes(sd_store* s, int64_t batch_index, void* out, int64_t cap, int64_t* out_len);
+/* device and host times of the calling thread's last sd_plan_update_store / sd_plan_delete_store (tools/mutation_bench.py):
+ * [0] scan kernels ms [1] sort ms [2] counting + writing merge ms [3] host install ms [4] whole statement ms (host clock) [5] rows */
+int sdx_last_mutation_timing(double out[6]);
 /* stats row (UnsafeRow) of a resident batch */
 int sdx_store_get_stats(sd_store* s, int64_t batch_index, void* out, int64_t cap, int64_t* out_len);
 int sdx_store_batch_info(sd_store* s, int64_t batch_index, int32_t* num_rows, int32_t* bucket_id,

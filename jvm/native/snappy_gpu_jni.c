@@ -232,6 +232,47 @@ JNIEXPORT void JNICALL JFN(planScanStore)(JNIEnv* env, jobject self, jlong plan,
   if (rc) throw_last(env);
 }
 
+/* ColumnUpdateExec / ColumnDeleteExec hand their statement over here: the WHERE and SET expressions are the plan's, the literal
+ * values an sd_literal array at literalsAddr (same layout as planSetLiterals); returns the number of rows changed */
+JNIEXPORT jlong JNICALL JFN(planUpdateStore)(JNIEnv* env, jobject self, jlong plan, jlong store, jintArray bucketIds,
+                                             jlong literalsAddr, jint nLiterals, jintArray targetCols) {
+  (void)self;
+  jint* ids = NULL;
+  jsize n = 0;
+  if (bucketIds != NULL) {
+    n = (*env)->GetArrayLength(env, bucketIds);
+    ids = (*env)->GetIntArrayElements(env, bucketIds, NULL);
+    if (ids == NULL) return 0;                               /* OutOfMemoryError is pending */
+  }
+  jint* tc = (*env)->GetIntArrayElements(env, targetCols, NULL);
+  if (tc == NULL) { if (ids) (*env)->ReleaseIntArrayElements(env, bucketIds, ids, JNI_ABORT); return 0; }
+  int64_t rows = 0;
+  int rc = sd_plan_update_store((sd_plan*)(intptr_t)plan, (sd_store*)(intptr_t)store, (const int32_t*)ids, (int32_t)n,
+                                (const sd_literal*)(intptr_t)literalsAddr, nLiterals, (const int32_t*)tc, &rows);
+  (*env)->ReleaseIntArrayElements(env, targetCols, tc, JNI_ABORT);
+  if (ids) (*env)->ReleaseIntArrayElements(env, bucketIds, ids, JNI_ABORT);
+  if (rc) throw_last(env);
+  return (jlong)rows;
+}
+
+JNIEXPORT jlong JNICALL JFN(planDeleteStore)(JNIEnv* env, jobject self, jlong plan, jlong store, jintArray bucketIds,
+                                             jlong literalsAddr, jint nLiterals) {
+  (void)self;
+  jint* ids = NULL;
+  jsize n = 0;
+  if (bucketIds != NULL) {
+    n = (*env)->GetArrayLength(env, bucketIds);
+    ids = (*env)->GetIntArrayElements(env, bucketIds, NULL);
+    if (ids == NULL) return 0;                               /* OutOfMemoryError is pending */
+  }
+  int64_t rows = 0;
+  int rc = sd_plan_delete_store((sd_plan*)(intptr_t)plan, (sd_store*)(intptr_t)store, (const int32_t*)ids, (int32_t)n,
+                                (const sd_literal*)(intptr_t)literalsAddr, nLiterals, &rows);
+  if (ids) (*env)->ReleaseIntArrayElements(env, bucketIds, ids, JNI_ABORT);
+  if (rc) throw_last(env);
+  return (jlong)rows;
+}
+
 /* ---- the cross-partition exchange (INTEGRATION.md section 4b) ------------------------------------------------------ */
 /* rank 0 fills a 128-byte id; the caller broadcasts it (a Spark broadcast variable) */
 JNIEXPORT void JNICALL JFN(commUniqueId)(JNIEnv* env, jobject self, jbyteArray out128) {

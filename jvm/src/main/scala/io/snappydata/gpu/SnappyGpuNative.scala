@@ -49,6 +49,12 @@ object SnappyGpuNative {
   /** scan the resident batches of these buckets (null: all) with the literals set by planSetLiterals; a store that has
     * grown since the plan's last scan is re-scanned incrementally (only the new batches get descriptors) */
   @native def planScanStore(plan: Long, store: Long, bucketIds: Array[Int]): Unit
+  /** UPDATE of the resident batches (ColumnUpdateExec): plan built with SD_PLAN_MUTATE, targetCols(i) = table ordinal that
+    * the plan's i-th projection writes, literals = sd_literal array at literalsAddr; returns the rows updated */
+  @native def planUpdateStore(plan: Long, store: Long, bucketIds: Array[Int], literalsAddr: Long, nLiterals: Int,
+      targetCols: Array[Int]): Long
+  /** DELETE of the resident rows the plan's filter matches (ColumnDeleteExec); returns the rows deleted */
+  @native def planDeleteStore(plan: Long, store: Long, bucketIds: Array[Int], literalsAddr: Long, nLiterals: Int): Long
 
   // ---- the exchange between co-located GPU partitions (INTEGRATION.md 4b) ------------------------------------------------
   /** rank 0 calls this and broadcasts the 128 bytes; every rank passes them to commCreate */

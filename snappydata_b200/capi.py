@@ -18,6 +18,7 @@ from .column_format import ColumnBatch, SqlType, parse_row_stream
 SD_ABI_VERSION = 2
 SD_NUM_METRICS = 12
 SD_OPT_RETAIN_BUFFERS = 1
+SD_PLAN_MUTATE = 1   # sd_plan_desc.flags: UPDATE / DELETE plan
 METRIC_NAMES = ["numOutputRows", "numRowsBuffer", "columnBatchesSeen", "updatedColumnCount",
                 "deletedBatchCount", "columnBatchesSkipped", "aggTimeNs", "kernelLaunches",
                 "rowsScanned", "algorithmicBytes", "h2dBytes", "scanOutputRows"]
@@ -225,6 +226,10 @@ class Api:
         self.host_free = fn("host_free", None, vp, required=False)
         self.plan_export_partials = fn("plan_export_partials", C.c_int, vp, vp, i64, required=False)
         self.plan_import_partials = fn("plan_import_partials", C.c_int, vp, vp, i64, required=False)
+        self.plan_update_store = fn("plan_update_store", C.c_int, vp, vp, C.POINTER(i32), i32, C.POINTER(sd_literal), i32,
+                                    C.POINTER(i32), C.POINTER(i64), required=False)
+        self.plan_delete_store = fn("plan_delete_store", C.c_int, vp, vp, C.POINTER(i32), i32, C.POINTER(sd_literal), i32,
+                                    C.POINTER(i64), required=False)
 
     def check(self, rc: int):
         if rc != 0:
@@ -255,13 +260,21 @@ def product_api() -> Api:
         L.sdx_store_batch_info.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
         L.sdx_store_memory_info.restype = C.c_int
         L.sdx_store_memory_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.sdx_store_get_delta.restype = C.c_int
+        L.sdx_store_get_delta.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
+        L.sdx_store_get_deletes.restype = C.c_int
+        L.sdx_store_get_deletes.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
+        L.sdx_last_mutation_timing.restype = C.c_int
+        L.sdx_last_mutation_timing.argtypes = [C.POINTER(C.c_double)]
     return _product
 
 
 class PlanDesc:
     """Owns the ctypes arrays behind an sd_plan_desc."""
 
-    def __init__(self, cols, exprs, filter_node, keys, aggs, proj, literal_types):
+    def __init__(self, cols, exprs, filter_node, keys, aggs, proj, literal_types, flags: int = 0, targets: Sequence[int] = ()):
+        self.flags = int(flags)              # SD_PLAN_MUTATE: UPDATE / DELETE
+        self.targets = list(targets)         # UPDATE: table ordinal that proj[i] writes
         self.cols_py = list(cols)            # (SqlType, nullable, table_ordinal[, scale])
         self.exprs_py = list(exprs)          # (op, type, a, b, c)
         self.keys_py = list(keys)
@@ -291,7 +304,7 @@ class PlanDesc:
         d.naggs, d.aggs = len(self.aggs_py), C.cast(self._aggs, C.POINTER(sd_agg))
         d.nproj, d.proj = len(self.proj_py), C.cast(self._proj, C.POINTER(C.c_int32))
         d.nliterals, d.literal_types = len(self.literal_types_py), C.cast(self._lt, C.POINTER(C.c_int32))
-        d.flags = 0
+        d.flags = self.flags
         self.c = d
 
     @property
@@ -454,6 +467,26 @@ class Plan:
             arr = (C.c_int32 * len(buckets))(*buckets)
             self.api.check(self.api.plan_scan_store(self.h, store.h, arr, len(buckets)))
         return self
+
+    def _mutation_args(self, store: "Store", lits: Sequence[object], buckets: Optional[Sequence[int]]):
+        arr = self.literal_array(lits)
+        b = (C.c_int32 * max(1, len(buckets or ())))(*(buckets or ()))
+        return arr, b, len(buckets or ())
+
+    def update_store(self, store: "Store", lits: Sequence[object] = (), buckets: Optional[Sequence[int]] = None) -> int:
+        """UPDATE store SET targets = proj WHERE filter, on the device (sd_plan_update_store) -> rows updated."""
+        arr, b, nb = self._mutation_args(store, lits, buckets)
+        tg = (C.c_int32 * max(1, len(self.desc.targets)))(*self.desc.targets)
+        rows = C.c_int64()
+        self.api.check(self.api.plan_update_store(self.h, store.h, b if nb else None, nb, arr, len(lits), tg, C.byref(rows)))
+        return int(rows.value)
+
+    def delete_store(self, store: "Store", lits: Sequence[object] = (), buckets: Optional[Sequence[int]] = None) -> int:
+        """DELETE FROM store WHERE filter, on the device (sd_plan_delete_store) -> rows deleted."""
+        arr, b, nb = self._mutation_args(store, lits, buckets)
+        rows = C.c_int64()
+        self.api.check(self.api.plan_delete_store(self.h, store.h, b if nb else None, nb, arr, len(lits), C.byref(rows)))
+        return int(rows.value)
 
     def finish_raw(self) -> bytes:
         while True:
@@ -660,3 +693,30 @@ class Store:
             self.close()
         except Exception:
             pass
+
+    def get_delta(self, batch_index: int, table_col: int, depth: int = 0) -> bytes:
+        """A resident update delta in the reference's byte layout (sdx_store_get_delta)."""
+        ln = C.c_int64()
+        rc = self.api.lib.sdx_store_get_delta(self.h, batch_index, table_col, depth, None, 0, C.byref(ln))
+        if rc not in (0, SD_ERR_OVERFLOW):
+            self.api.check(rc)
+        buf = C.create_string_buffer(max(1, ln.value))
+        self.api.check(self.api.lib.sdx_store_get_delta(self.h, batch_index, table_col, depth, buf, len(buf), C.byref(ln)))
+        return buf.raw[: ln.value]
+
+    def get_deletes(self, batch_index: int) -> bytes:
+        """A batch's delete mask [0][numBaseRows][numDeletes][positions] (sdx_store_get_deletes)."""
+        ln = C.c_int64()
+        rc = self.api.lib.sdx_store_get_deletes(self.h, batch_index, None, 0, C.byref(ln))
+        if rc not in (0, SD_ERR_OVERFLOW):
+            self.api.check(rc)
+        buf = C.create_string_buffer(max(1, ln.value))
+        self.api.check(self.api.lib.sdx_store_get_deletes(self.h, batch_index, buf, len(buf), C.byref(ln)))
+        return buf.raw[: ln.value]
+
+
+def last_mutation_timing(api: Api) -> Dict[str, float]:
+    """Device and host times of the calling thread's last UPDATE / DELETE (sdx_last_mutation_timing)."""
+    out = (C.c_double * 6)()
+    api.check(api.lib.sdx_last_mutation_timing(out))
+    return dict(zip(("scan_ms", "sort_ms", "merge_ms", "install_ms", "statement_ms", "rows"), list(out)))

@@ -109,6 +109,7 @@ sd_plan_desc PlanSpec::desc_view() const {
   d.naggs = (int)aggs.size(); d.aggs = aggs.data();
   d.nproj = (int)proj.size(); d.proj = proj.data();
   d.nliterals = (int)literal_types.size(); d.literal_types = literal_types.data();
+  d.flags = flags;
   return d;
 }
 
@@ -576,7 +577,7 @@ struct Gen {
       grp << "    return " << g << ";\n";
     } else grp << "    return 0;\n";
     std::ostringstream projfn;
-    if (p.mode == MODE_PROJECT) {
+    if (p.mode == MODE_PROJECT || p.mode == MODE_MUTATE) {   // MODE_MUTATE: the SET values of an UPDATE (none for a DELETE)
       std::fill(done.begin(), done.end(), 0);
       sig << ";proj=";
       for (size_t j = 0; j < p.proj.size(); j++) {
@@ -658,7 +659,7 @@ struct Gen {
     o << "// signature: " << p.signature << "\n";
     o << "struct " << p.struct_name << " {\n";
     o << "  static constexpr int NC = " << nc << ";\n  static constexpr int NSLOT = " << ns << ";\n";
-    o << "  static constexpr int MODE = " << (p.mode == MODE_GROUPS ? "sd::MODE_GROUPS" : p.mode == MODE_HASH ? "sd::MODE_HASH" : p.mode == MODE_PROJECT ? "sd::MODE_PROJECT" : "sd::MODE_NOKEY") << ";\n";
+    o << "  static constexpr int MODE = " << (p.mode == MODE_GROUPS ? "sd::MODE_GROUPS" : p.mode == MODE_HASH ? "sd::MODE_HASH" : p.mode == MODE_PROJECT ? "sd::MODE_PROJECT" : p.mode == MODE_MUTATE ? "sd::MODE_MUTATE" : "sd::MODE_NOKEY") << ";\n";
     o << "  static constexpr int NKEYS = " << p.keys.size() << ";\n";
     o << "  static constexpr int NPROJ = " << p.proj.size() << ";\n";
     o << "  static constexpr int MIN_CTAS = " << p.min_ctas << ";\n  static constexpr int RPT = " << p.rpt << ";\n";
@@ -714,13 +715,16 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
   out.proj.assign(d->proj, d->proj + d->nproj);
   out.literal_types.assign(d->literal_types, d->literal_types + d->nliterals);
   out.filter = d->filter;
+  const bool mutate = (d->flags & SD_PLAN_MUTATE) != 0;
+  out.flags = mutate ? SD_PLAN_MUTATE : 0;
   Gen g(out, err);
   int rc = g.validate();
   if (rc) return rc;
   for (auto& c : out.cols) out.kinds.push_back(kind_of_type(c.type));
   g.nullability();
   const bool projection = out.aggs.empty() && out.keys.empty();
-  if (projection && out.proj.empty()) { err = "plan has neither aggregates nor projection columns"; return SD_ERR_INVALID; }
+  if (mutate && !projection) { err = "an UPDATE / DELETE plan has no grouping keys and no aggregates"; return SD_ERR_INVALID; }
+  if (projection && out.proj.empty() && !mutate) { err = "plan has neither aggregates nor projection columns"; return SD_ERR_INVALID; }
   if (projection) {
     if (out.proj.size() > 32) { err = "more than 32 projected columns"; return SD_ERR_UNSUPPORTED; }
     for (int n : out.proj) {
@@ -728,7 +732,7 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
       if (e.type == SD_STRING && e.op != SD_OP_COL) { err = "projected STRING expression that is not a dictionary column"; return SD_ERR_UNSUPPORTED; }
     }
   }
-  out.mode = projection ? MODE_PROJECT : MODE_NOKEY;
+  out.mode = mutate ? MODE_MUTATE : projection ? MODE_PROJECT : MODE_NOKEY;
   if (!out.keys.empty()) {
     bool all_dict_strings = true;
     for (int k : out.keys) {

@@ -62,6 +62,7 @@ struct PlanSpec {
   std::vector<int32_t> proj;
   std::vector<int32_t> literal_types;
   int filter = -1;
+  int flags = 0;                     // sd_plan_desc.flags (SD_PLAN_MUTATE)
   // analysis
   std::vector<int> expr_nullable;
   std::vector<int> kinds;            // K_* per scan column
@@ -69,7 +70,7 @@ struct PlanSpec {
   std::vector<SlotSpec> slots;
   std::vector<AggMap> agg_map;
   int rows_slot = -1;                // COUNT(*)-like slot that tells which groups exist
-  int mode = 0;                      // MODE_NOKEY | MODE_GROUPS | MODE_HASH
+  int mode = 0;                      // MODE_NOKEY | MODE_GROUPS | MODE_HASH | MODE_PROJECT | MODE_MUTATE
   int rpt = 4;                       // rows per thread per tile (2, 4, 8)
   int min_ctas = 2;                  // __launch_bounds__ min CTAs per SM (= target CTAs per SM)
   int stages = 1;                    // > 0: staged fast path (producer warp + cp.async.bulk ring); 0: direct loads

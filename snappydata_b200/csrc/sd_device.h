@@ -122,7 +122,10 @@ struct Literals {
 //   MODE_PROJECT no aggregate: rows that pass the filter are emitted as fixed-width records
 //               [uint32 batch][uint32 null bits][8 bytes x NPROJ] (strings as dictionary codes; the host
 //               turns records into UnsafeRows)
-enum : int32_t { MODE_NOKEY = 0, MODE_GROUPS = 1, MODE_HASH = 2, MODE_PROJECT = 3 };
+//   MODE_MUTATE  UPDATE / DELETE (SD_PLAN_MUTATE): every live row that passes the WHERE becomes a record
+//               [uint64 batch << 32 | row][uint64 null bits][8 bytes x max(NPROJ, 1)] -- the first word is the
+//               (batch, row) sort key of the merge that follows (sd_mutate.cu)
+enum : int32_t { MODE_NOKEY = 0, MODE_GROUPS = 1, MODE_HASH = 2, MODE_PROJECT = 3, MODE_MUTATE = 4 };
 
 // Device hash table of MODE_HASH: entry e = state[e] (0 empty, 1 being written, 2 full), keys[e][NK] (int64 codes),
 // knull[e] (bit k: key k is NULL), vals[e][NSLOT].

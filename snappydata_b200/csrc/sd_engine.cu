@@ -660,7 +660,7 @@ int hash_ensure(sd_plan* p, uint32_t capacity) {
 }
 
 int ensure_out(sd_plan* p, int64_t cap_records) {
-  const int64_t rec = 8 + 8 * (int64_t)std::max<size_t>(p->spec.proj.size(), 1);
+  const int64_t rec = (p->spec.mode == MODE_MUTATE ? 16 : 8) + 8 * (int64_t)std::max<size_t>(p->spec.proj.size(), 1);
   if (!p->d_out_count) { SD_CUDA(cudaMalloc(&p->d_out_count, 64)); SD_CUDA(cudaMemset(p->d_out_count, 0, 64)); }
   if (cap_records > p->out_cap) {
     if (p->d_out) cudaFree(p->d_out);
@@ -836,7 +836,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   if (sp.mode == MODE_HASH) {
     int rc = hash_ensure(p, p->hash_capacity ? p->hash_capacity : (1u << 16));
     if (rc) return rc;
-  } else if (sp.mode == MODE_PROJECT) {
+  } else if (sp.mode == MODE_PROJECT || sp.mode == MODE_MUTATE) {
     int rc = ensure_out(p, p->out_cap ? p->out_cap : (int64_t(1) << 20));
     if (rc) return rc;
   } else if (!p->result_init) {
@@ -1533,6 +1533,7 @@ const char* sd_plan_kernel_name(sd_plan* p) { return p ? p->kernel_name.c_str() 
 int sd_batch_submit(sd_plan* p, const sd_batch* b) {
   if (!p || !b) return set_error(SD_ERR_INVALID, "sd_batch_submit: null argument");
   if (!p->lits_set) return set_error(SD_ERR_STATE, "sd_batch_submit: literals not set");
+  if (p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_batch_submit: an UPDATE / DELETE plan runs over a resident store only");
   if (b->ncols != (int)p->spec.cols.size()) return set_error(SD_ERR_INVALID, "sd_batch_submit: batch has %d columns, plan scans %zu", b->ncols, p->spec.cols.size());
   SD_CUDA(cudaSetDevice(p->device));
   p->metrics[2]++;   // columnBatchesSeen
@@ -1563,8 +1564,58 @@ int sd_batch_submit(sd_plan* p, const sd_batch* b) {
   return 0;
 }
 
+static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets);
+
 int sd_plan_scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets) {
   if (!p || !s) return set_error(SD_ERR_INVALID, "sd_plan_scan_store: null argument");
+  if (p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_scan_store: an UPDATE / DELETE plan runs through sd_plan_update_store / sd_plan_delete_store");
+  return scan_store(p, s, bucket_ids, nbuckets);
+}
+
+}  // extern "C"
+
+const PlanSpec& sd::plan_spec(const sd_plan* p) { return p->spec; }
+
+// The scan of an UPDATE / DELETE statement (sd_mutate.cu merges what it finds): the plan's records over the store's current
+// batches -- the same staged ring, overlay path, stats skipping and grow-and-replay as a projection -- left on the device.
+int sd::mutation_scan(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, const sd_literal* lits, int32_t nlits,
+                      MutationScan* out) {
+  if (p->spec.mode != MODE_MUTATE) return set_error(SD_ERR_STATE, "not an UPDATE / DELETE plan (sd_plan_desc.flags lacks SD_PLAN_MUTATE)");
+  int rc = sd_plan_reset(p);
+  if (rc) return rc;
+  rc = sd_plan_set_literals(p, lits, nlits);
+  if (rc) return rc;
+  rc = scan_store(p, s, bucket_ids, nbuckets);
+  if (rc) return rc;
+  rc = ensure_out(p, p->out_cap ? p->out_cap : 1024);
+  if (rc) return rc;
+  unsigned long long count = 0;
+  for (;;) {   // the one read-back of the scan: how many rows matched (grow + replay when the record buffer was too small)
+    SD_CUDA(cudaMemcpyAsync(&count, p->d_out_count, 8, cudaMemcpyDeviceToHost, p->stream));
+    SD_CUDA(cudaStreamSynchronize(p->stream));
+    if ((int64_t)count <= p->out_cap) break;
+    rc = ensure_out(p, (int64_t)count + (int64_t)count / 8 + 1024);
+    if (rc) return rc;
+    SD_CUDA(cudaMemsetAsync(p->d_out_count, 0, 8, p->stream));
+    SD_CUDA(cudaMemsetAsync(p->d_counters, 0, 64, p->stream));
+    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, nullptr, l.batch_base); if (rc) return rc; }
+  }
+  update_agg_time(p);
+  p->metrics[6] = (int64_t)(p->agg_ms * 1e6);
+  out->records = reinterpret_cast<const uint64_t*>(p->d_out);
+  out->count = (int64_t)count;
+  out->rec_words = 2 + (int)std::max<size_t>(p->spec.proj.size(), 1);
+  out->batches = p->exec_batches;
+  out->stream = p->stream;
+  out->scan_ms = p->agg_ms;
+  p->finished_nrows = (int64_t)count;
+  p->metrics[0] = (int64_t)count;
+  return 0;
+}
+
+extern "C" {
+
+static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets) {
   if (!p->lits_set) return set_error(SD_ERR_STATE, "sd_plan_scan_store: literals not set");
   if (s->device != p->device) return set_error(SD_ERR_INVALID, "store lives on device %d, plan on %d", s->device, p->device);
   SD_CUDA(cudaSetDevice(p->device));
@@ -1600,6 +1651,7 @@ int sd_plan_scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32
     for (size_t i = from; i < snapshot.size(); i++) {
       const StoredBatch& sb = *snapshot[i];
       if (!buckets.empty() && std::find(buckets.begin(), buckets.end(), sb.bucket_id) == buckets.end()) continue;
+      if (sb.gone) continue;   // every row deleted (ColumnDelta.checkBatchDeleted): not a batch any more
       (*seen)++;
       if (!batch_passes_stats(p, sb)) { (*skipped)++; continue; }
       list.push_back(&sb);
@@ -1631,6 +1683,7 @@ int sd_plan_scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32
         for (size_t i = 0; i < keep; i++) {
           const StoredBatch& sb = *snapshot[i];
           if (!buckets.empty() && std::find(buckets.begin(), buckets.end(), sb.bucket_id) == buckets.end()) continue;
+          if (sb.gone) continue;
           seen0++;
         }
         skipped0 = seen0 - (int64_t)c.segs[0].batches.size();
@@ -1771,6 +1824,7 @@ static int collect_partial_rows(sd_plan* p) {
 }
 
 int sd_plan_finish(sd_plan* p, void* out_rows, int64_t cap, int64_t* out_len, int64_t* out_nrows) {
+  if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_finish: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !out_len) return set_error(SD_ERR_INVALID, "sd_plan_finish: null argument");
   int rc = collect_partial_rows(p);
   if (rc) return rc;
@@ -1857,6 +1911,7 @@ void sd_plan_destroy(sd_plan* p) {
 
 // ---- dense partial table export/import for an on-device exchange (NCCL all-reduce) --------------
 int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32_t* slot_is_f64) {
+  if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_partials_layout: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
   const int ns = (int)p->spec.slots.size();
   if (ngroups) *ngroups = p->ngroups;
@@ -1865,6 +1920,7 @@ int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32
   return 0;
 }
 int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes) {
+  if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_export_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_out) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
   SD_CUDA(cudaSetDevice(p->device));
@@ -1877,6 +1933,7 @@ int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes) {
   return 0;
 }
 int sd_plan_import_partials(sd_plan* p, const void* dev_in, int64_t bytes) {
+  if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_import_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_in) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
   p->finished_nrows = -1;
@@ -2225,6 +2282,7 @@ static bool dense_exchange_eligible(const sd_plan* p) {
 }
 
 int sd_plan_exchange(sd_plan* p, sd_comm* c) {
+  if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_exchange: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !c) return set_error(SD_ERR_INVALID, "sd_plan_exchange: null argument");
   if (c->device != p->device) return set_error(SD_ERR_INVALID, "communicator lives on device %d, plan on %d", c->device, p->device);
   static thread_local LapStats laps;

@@ -137,6 +137,8 @@ struct StoredDelta {
   bool present = false;
   DevDelta dev;                           // device pointers
   int64_t len = 0;
+  int32_t nbase = 0;                      // numBaseRows of the header
+  int64_t body_off = 0;                   // offset of the values (dictionary) in the reference layout
   std::vector<std::string> dict_strings;  // STRING values dictionary
 };
 
@@ -171,6 +173,7 @@ struct StoredBatch {
   int32_t num_deletes = 0;
   bool has_deltas = false;
   bool positional = false;                // cols are indexed by the plan's scan column (private store)
+  bool gone = false;                      // every row deleted (ColumnDelta.checkBatchDeleted): no scan reads it
 };
 
 }  // namespace sd
@@ -190,6 +193,10 @@ struct sd_store {
   int next_stream = 0;
   cudaEvent_t extra_done[4] = {nullptr, nullptr, nullptr, nullptr};
   std::vector<std::unique_ptr<sd::StoredBatch>> batches;
+  // UPDATE / DELETE replace a batch by a new version at the same index; the old one stays alive here until the store is
+  // destroyed (scans hold raw pointers into their snapshot).  `mutate_mu` serialises the statements on this store.
+  std::vector<std::unique_ptr<sd::StoredBatch>> retired;
+  std::mutex mutate_mu;
   int64_t version = 0;
   int64_t h2d_bytes = 0;
   bool retain_buffers = false;   // SD_OPT_RETAIN_BUFFERS: no per-put synchronisation of the copy stream
@@ -225,6 +232,21 @@ int store_flush_lz4(sd_store* s);
 int store_lz4_order(sd_store* s, cudaStream_t stream);
 // block until the queued expansions are done, release their staging memory, report a corrupt payload
 int store_lz4_check(sd_store* s);
+
+// records of an UPDATE / DELETE scan, on the device (sd_engine.cu; merged by sd_mutate.cu): `count` records of `rec_words`
+// uint64 words, [batch << 32 | row][null bits][SET values]; the batch ordinal indexes `batches`
+struct MutationScan {
+  const uint64_t* records = nullptr;
+  int64_t count = 0;
+  int rec_words = 0;
+  std::vector<const StoredBatch*> batches;
+  cudaStream_t stream = nullptr;
+  float scan_ms = 0;
+};
+int mutation_scan(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, const sd_literal* lits, int32_t nlits,
+                  MutationScan* out);
+// the analysed plan of a handle (sd_engine.cu)
+const PlanSpec& plan_spec(const sd_plan* p);
 }
 
 #endif

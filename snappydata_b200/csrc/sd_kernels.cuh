@@ -1062,7 +1062,7 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   } else if (PLAN::MODE == MODE_NOKEY) {
 #pragma unroll
     for (int s = 0; s < NSLOT; s++) acc[s] = slot_identity(PLAN::slot_op(s));
-  } else if (PLAN::MODE == MODE_HASH || PLAN::MODE == MODE_PROJECT) {
+  } else if (PLAN::MODE == MODE_HASH || PLAN::MODE == MODE_PROJECT || PLAN::MODE == MODE_MUTATE) {
     // nothing per CTA: the table / output buffer is global
   } else if (args.table_mode == TABLE_PRIVATE) {
     // private table of thread t: entry e at table[e * THREADS + t]: lanes hit distinct banks
@@ -1163,10 +1163,11 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
 
       // ---- row at a time over registers: filter -> group -> accumulate -------------------------
       c_scanned += __popc(live);
-      if (PLAN::MODE == MODE_PROJECT) {
+      if (PLAN::MODE == MODE_PROJECT || PLAN::MODE == MODE_MUTATE) {
         // filter -> project: passing rows become fixed-width records; one atomic per warp per row slot
         constexpr int NP = PLAN::NPROJ > 0 ? PLAN::NPROJ : 1;
-        constexpr int REC = 8 + 8 * NP;
+        constexpr int HDR = PLAN::MODE == MODE_MUTATE ? 2 : 1;   // MODE_MUTATE: (batch, row) key word + null word
+        constexpr int REC = 8 * HDR + 8 * NP;
 #pragma unroll
         for (int r = 0; r < RPT; r++) {
           bool pass = false;
@@ -1189,9 +1190,14 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
               const unsigned long long idx = base + __popc(m & ((1u << lane_id) - 1u));
               if ((int64_t)idx < args.out_cap) {
                 uint64_t* rec = reinterpret_cast<uint64_t*>(args.out_rows + idx * REC);
-                rec[0] = (uint64_t)(uint32_t)(args.batch_base + lo) | ((uint64_t)pnull << 32);
+                if (PLAN::MODE == MODE_MUTATE) {
+                  rec[0] = ((uint64_t)(uint32_t)(args.batch_base + lo) << 32) | (uint32_t)(tile_start + row_in_tile(r));
+                  rec[1] = pnull;
+                } else {
+                  rec[0] = (uint64_t)(uint32_t)(args.batch_base + lo) | ((uint64_t)pnull << 32);
+                }
 #pragma unroll
-                for (int j = 0; j < PLAN::NPROJ; j++) rec[1 + j] = pv[j];
+                for (int j = 0; j < PLAN::NPROJ; j++) rec[HDR + j] = pv[j];
               }
             }
           }
@@ -1252,7 +1258,7 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   consumer_sync();
   uint64_t* my_partials = args.partials + (size_t)blockIdx.x * NE;
   const int lane = tid & 31, warp = tid >> 5;
-  if (PLAN::MODE == MODE_HASH || PLAN::MODE == MODE_PROJECT) {
+  if (PLAN::MODE == MODE_HASH || PLAN::MODE == MODE_PROJECT || PLAN::MODE == MODE_MUTATE) {
     // results live in the global hash table / the output record buffer
   } else if (PLAN::MODE == MODE_NOKEY) {
     uint64_t* scratch = table;   // [NSLOT][THREADS/32]
@@ -1307,7 +1313,7 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   consumer_sync();
   if (tid == 0) is_last = atomicAdd(args.ticket, 1u) == gridDim.x - 1;
   consumer_sync();
-  if (is_last && PLAN::MODE != MODE_HASH && PLAN::MODE != MODE_PROJECT && !(PLAN::MODE == MODE_GROUPS && args.table_mode == TABLE_GLOBAL_ATOMIC)) {
+  if (is_last && PLAN::MODE != MODE_HASH && PLAN::MODE != MODE_PROJECT && PLAN::MODE != MODE_MUTATE && !(PLAN::MODE == MODE_GROUPS && args.table_mode == TABLE_GLOBAL_ATOMIC)) {
     __threadfence();
     for (int e = tid; e < NE; e += THREADS) {
       const int op = PLAN::slot_op_rt(e % NSLOT);

@@ -562,6 +562,8 @@ static int upload_delta(sd_store* s, const uint8_t* buf, int64_t len, int type, 
   d = StoredDelta();
   d.present = true;
   d.len = len;
+  d.nbase = rd_i32(cpos);
+  d.body_off = data_off;
   memset(&d.dev, 0, sizeof(d.dev));
   d.dev.n = n; d.dev.enc = type_id; d.dev.nwords = null_bytes >> 3;
   uint8_t* p = nullptr;

@@ -8,9 +8,9 @@ one compiled plan serves every literal value.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
-from .capi import AggFn, Op, PlanDesc
+from .capi import SD_PLAN_MUTATE, AggFn, Op, PlanDesc
 from .column_format import SqlType
 
 _NUMERIC_RANK = {SqlType.BYTE: 1, SqlType.SHORT: 2, SqlType.INT: 3, SqlType.LONG: 4, SqlType.FLOAT: 5, SqlType.DOUBLE: 6}
@@ -72,6 +72,8 @@ class PlanBuilder:
         self._keys: List[E] = []
         self._aggs: List[Tuple[int, Optional[E]]] = []
         self._proj: List[E] = []
+        self._flags = 0
+        self._targets: List[int] = []
 
     # scan columns (ColumnTableScan.output)
     def col(self, t: SqlType, table_ordinal: int, nullable: bool = False, scale: int = 0, precision: int = 0) -> E:
@@ -101,6 +103,18 @@ class PlanBuilder:
     def count(self, e: Optional[E] = None): return self.agg(AggFn.COUNT if e is not None else AggFn.COUNT_STAR, e)
     def project(self, *es: E): self._proj = list(es); return self
 
+    # UPDATE / DELETE over a resident store (SD_PLAN_MUTATE; the WHERE clause is filter())
+    def update(self, assignments: Dict[int, E]):
+        """UPDATE ... SET table column k = assignments[k], ...: the values become the plan's projection."""
+        self._targets = [int(k) for k in assignments]
+        self._proj = [assignments[k] for k in assignments]
+        self._flags = SD_PLAN_MUTATE
+        return self
+
+    def delete(self):
+        self._targets, self._proj, self._flags = [], [], SD_PLAN_MUTATE
+        return self
+
     def build(self) -> PlanDesc:
         nodes: List[Tuple[int, int, int, int, int]] = []
         memo = {}
@@ -126,7 +140,7 @@ class PlanBuilder:
         keys = [emit(k) for k in self._keys]
         aggs = [(fn, emit(e) if e is not None else -1) for fn, e in self._aggs]
         proj = [emit(p) for p in self._proj]
-        return PlanDesc(self.cols, nodes, f, keys, aggs, proj, self.literal_types)
+        return PlanDesc(self.cols, nodes, f, keys, aggs, proj, self.literal_types, self._flags, self._targets)
 
 
 # ---- the benchmark plans ------------------------------------------------------------------------
