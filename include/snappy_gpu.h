@@ -272,6 +272,24 @@ int sd_plan_update_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int
 int sd_plan_delete_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, const sd_literal* lits, int32_t nlits,
                          int64_t* rows_deleted);
 
+/* ---- compaction on the device: fold the update deltas and delete masks of resident batches back into their base columns.
+ *      Rewrites the dirty resident batches of the given buckets (NULL/0 = all) without their update deltas and delete masks.
+ *      A batch is dirty when it carries a delta or a delete mask.  It is selected when
+ *        (deleted rows + delta entries of its resident columns, depth 0 and 1) >= min_dirty_fraction * num_rows;
+ *      min_dirty_fraction = 0 selects every dirty batch.  A batch whose every row is deleted is removed from the store.
+ *      Every column of a selected batch that has a delta is rewritten -- every resident column when the batch has a delete
+ *      mask -- as the bytes sd_store_encode_batch writes for the batch's live rows with their current values, in their
+ *      original order, in the type's default encoding; other columns keep their bytes.  Rewritten columns get the encoder's
+ *      stats entries, the row count becomes the live rows.  The new version keeps bucket_id and batch_id, gets a new identity
+ *      and has no deltas and no mask: its row ordinals are the live rows renumbered from 0, and later UPDATE / DELETE
+ *      statements address those.  Serialised with UPDATE / DELETE; works on the batches present when it starts; everything
+ *      is installed in one step under the store's lock (a scan sees all of it or none).  Superseded bytes stay in the arena
+ *      until the store is destroyed.  Refused with nothing installed: a column that must be rewritten but that the engine
+ *      cannot decode -- an Uncompressed (variable-width) STRING column, a column the scan does not support --
+ *      (SD_ERR_UNSUPPORTED, naming batch and column); a negative or NaN min_dirty_fraction, a null store (SD_ERR_INVALID).
+ *      out[0] batches rewritten, out[1] batches removed, out[2] deleted rows purged, out[3] bytes written to the store's arena */
+int sd_store_compact(sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, double min_dirty_fraction, int64_t out[4]);
+
 /* ---- final merge (SnappyHashAggregateExec(Final) / CollectAggregateExec.executeCollect,
  *      core/execution/aggregate/CollectAggregateExec.scala:67-121): merges partial rows of all
  *      partitions (sums add, counts add, min/max combine) and evaluates results (avg = sum/count).
@@ -340,6 +358,9 @@ int sdx_store_get_deletes(sd_store* s, int64_t batch_index, void* out, int64_t c
 /* device and host times of the calling thread's last sd_plan_update_store / sd_plan_delete_store (tools/mutation_bench.py):
  * [0] scan kernels ms [1] sort ms [2] counting + writing merge ms [3] host install ms [4] whole statement ms (host clock) [5] rows */
 int sdx_last_mutation_timing(double out[6]);
+/* the calling thread's last sd_store_compact: [0] materialise ms [1] encode ms (device events) [2] host layout + install ms
+ * [3] whole call ms (host clock) [4] rows of the rewritten batches [5] bytes read (columns, deltas, delete masks) */
+int sdx_last_compaction_timing(double out[6]);
 /* stats row (UnsafeRow) of a resident batch */
 int sdx_store_get_stats(sd_store* s, int64_t batch_index, void* out, int64_t cap, int64_t* out_len);
 int sdx_store_batch_info(sd_store* s, int64_t batch_index, int32_t* num_rows, int32_t* bucket_id,

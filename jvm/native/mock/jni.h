@@ -9,6 +9,7 @@
 typedef int32_t jint;
 typedef int64_t jlong;
 typedef int8_t jbyte;
+typedef double jdouble;
 typedef uint8_t jboolean;
 typedef jint jsize;
 struct _jobject;

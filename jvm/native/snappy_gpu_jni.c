@@ -273,6 +273,30 @@ JNIEXPORT jlong JNICALL JFN(planDeleteStore)(JNIEnv* env, jobject self, jlong pl
   return (jlong)rows;
 }
 
+/* compaction: folds update deltas and delete masks back into the base columns (sd_store_compact); out (length >= 4):
+ * batches rewritten, batches removed, deleted rows purged, bytes written to the store's arena */
+JNIEXPORT void JNICALL JFN(compactStore)(JNIEnv* env, jobject self, jlong store, jintArray bucketIds, jdouble minDirtyFraction,
+                                         jlongArray out) {
+  (void)self;
+  if (out == NULL || (*env)->GetArrayLength(env, out) < 4) {
+    throw_msg(env, "java/lang/IllegalArgumentException", "compactStore: out must hold 4 longs");
+    return;
+  }
+  jint* ids = NULL;
+  jsize n = 0;
+  if (bucketIds != NULL) {
+    n = (*env)->GetArrayLength(env, bucketIds);
+    ids = (*env)->GetIntArrayElements(env, bucketIds, NULL);
+    if (ids == NULL) return;                                  /* OutOfMemoryError is pending */
+  }
+  int64_t counts[4] = {0, 0, 0, 0};
+  int rc = sd_store_compact((sd_store*)(intptr_t)store, (const int32_t*)ids, (int32_t)n, (double)minDirtyFraction, counts);
+  if (ids) (*env)->ReleaseIntArrayElements(env, bucketIds, ids, JNI_ABORT);
+  if (rc) { throw_last(env); return; }
+  jlong o[4] = {(jlong)counts[0], (jlong)counts[1], (jlong)counts[2], (jlong)counts[3]};
+  (*env)->SetLongArrayRegion(env, out, 0, 4, o);
+}
+
 /* ---- the cross-partition exchange (INTEGRATION.md section 4b) ------------------------------------------------------ */
 /* rank 0 fills a 128-byte id; the caller broadcasts it (a Spark broadcast variable) */
 JNIEXPORT void JNICALL JFN(commUniqueId)(JNIEnv* env, jobject self, jbyteArray out128) {

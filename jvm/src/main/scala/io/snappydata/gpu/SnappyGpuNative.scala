@@ -55,6 +55,11 @@ object SnappyGpuNative {
       targetCols: Array[Int]): Long
   /** DELETE of the resident rows the plan's filter matches (ColumnDeleteExec); returns the rows deleted */
   @native def planDeleteStore(plan: Long, store: Long, bucketIds: Array[Int], literalsAddr: Long, nLiterals: Int): Long
+  /** folds update deltas and delete masks of the store's dirty batches (bucketIds null = all) back into their base columns;
+    * batches with (deleted rows + delta entries) >= minDirtyFraction * rows are rewritten, fully deleted ones removed.
+    * out(0) batches rewritten, out(1) removed, out(2) deleted rows purged, out(3) bytes written.  Rewritten batches number
+    * their live rows from 0: later UPDATE / DELETE positions and any JVM-side mirror of the bytes follow the new version */
+  @native def compactStore(store: Long, bucketIds: Array[Int], minDirtyFraction: Double, out: Array[Long]): Unit
 
   // ---- the exchange between co-located GPU partitions (INTEGRATION.md 4b) ------------------------------------------------
   /** rank 0 calls this and broadcasts the 128 bytes; every rank passes them to commCreate */

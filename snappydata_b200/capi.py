@@ -266,6 +266,10 @@ def product_api() -> Api:
         L.sdx_store_get_deletes.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
         L.sdx_last_mutation_timing.restype = C.c_int
         L.sdx_last_mutation_timing.argtypes = [C.POINTER(C.c_double)]
+        L.sd_store_compact.restype = C.c_int
+        L.sd_store_compact.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_double, C.POINTER(C.c_int64)]
+        L.sdx_last_compaction_timing.restype = C.c_int
+        L.sdx_last_compaction_timing.argtypes = [C.POINTER(C.c_double)]
     return _product
 
 
@@ -704,6 +708,15 @@ class Store:
         self.api.check(self.api.lib.sdx_store_get_delta(self.h, batch_index, table_col, depth, buf, len(buf), C.byref(ln)))
         return buf.raw[: ln.value]
 
+    def compact(self, min_dirty_fraction: float = 0.0, buckets: Optional[Sequence[int]] = None) -> Dict[str, int]:
+        """Fold the update deltas and delete masks of dirty batches back into their base columns, on the device
+        (sd_store_compact).  Rewritten batches number their live rows from 0; fully deleted batches leave the store."""
+        nb = len(buckets or ())
+        b = (C.c_int32 * max(1, nb))(*(buckets or ()))
+        out = (C.c_int64 * 4)()
+        self.api.check(self.api.lib.sd_store_compact(self.h, b if nb else None, nb, float(min_dirty_fraction), out))
+        return dict(zip(("batches_rewritten", "batches_removed", "rows_purged", "bytes_written"), (int(x) for x in out)))
+
     def get_deletes(self, batch_index: int) -> bytes:
         """A batch's delete mask [0][numBaseRows][numDeletes][positions] (sdx_store_get_deletes)."""
         ln = C.c_int64()
@@ -720,3 +733,10 @@ def last_mutation_timing(api: Api) -> Dict[str, float]:
     out = (C.c_double * 6)()
     api.check(api.lib.sdx_last_mutation_timing(out))
     return dict(zip(("scan_ms", "sort_ms", "merge_ms", "install_ms", "statement_ms", "rows"), list(out)))
+
+
+def last_compaction_timing(api: Api) -> Dict[str, float]:
+    """Device and host times of the calling thread's last compaction (sdx_last_compaction_timing)."""
+    out = (C.c_double * 6)()
+    api.check(api.lib.sdx_last_compaction_timing(out))
+    return dict(zip(("materialise_ms", "encode_ms", "host_ms", "compaction_ms", "rows_read", "bytes_read"), list(out)))

@@ -15,10 +15,12 @@
 // Work split: the device does everything that touches every row (null words, compaction of the non-null values, the boolean
 // bit set, finding the distinct strings and their first occurrence, rewriting strings as dictionary indexes, min / max);
 // the host only lays out the buffer (header, trimmed null words, the dictionary in first-seen order) from a few KB of
-// feedback.
+// feedback.  The phases after the raw values are on the device (enc_null_words_many / enc_queue_words / enc_first_seen_dict / enc_layout / enc_write, declared in
+// sd_host.h) are shared with compaction (sd_compact.cu), which feeds them the materialised columns of many batches at once.
 #include <algorithm>
 #include <climits>
 #include <cstring>
+#include <functional>
 
 #include "sd_host.h"
 
@@ -43,14 +45,20 @@ struct EncCol {
   int32_t n;
 };
 
-__global__ void enc_null_words_kernel(const uint8_t* nulls, int n, uint64_t* words, int* fb /* [0] nulls, [1] last non-zero word + 1 */) {
-  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void null_word(const uint8_t* nulls, int n, uint64_t* words, int* fb, int w) {
   if ((int64_t)w * 64 >= n) return;
   uint64_t word = 0;
   const int lim = min(64, n - w * 64);
   for (int b = 0; b < lim; b++) word |= (uint64_t)(nulls[(int64_t)w * 64 + b] != 0) << b;
   words[w] = word;
   if (word) { atomicAdd(&fb[0], __popcll(word)); atomicMax(&fb[1], w + 1); }
+}
+// the null words of many columns in one launch (fb: [0] nulls, [1] last non-zero word + 1): blockIdx.y = column, a
+// grid-stride loop over its words
+struct NullJob { const uint8_t* nulls; uint64_t* words; int* fb; int n; int pad_; };
+__global__ void enc_null_words_many_kernel(const NullJob* jobs) {
+  const NullJob j = jobs[blockIdx.y];
+  for (int w = blockIdx.x * blockDim.x + threadIdx.x; (int64_t)w * 64 < j.n; w += gridDim.x * blockDim.x) null_word(j.nulls, j.n, j.words, j.fb, w);
 }
 
 template <class T> __device__ __forceinline__ T ld_raw(const uint8_t* p, int64_t i) { return reinterpret_cast<const T*>(p)[i]; }
@@ -191,45 +199,188 @@ int kind_of(int t) {
 }
 void put32(std::vector<uint8_t>& b, int32_t v) { b.insert(b.end(), reinterpret_cast<uint8_t*>(&v), reinterpret_cast<uint8_t*>(&v) + 4); }
 
-// stats UnsafeRow [count:int][(lower, upper, nullCount:int) per table column] (enc/ColumnEncoding.scala:1015-1036)
-struct ColStat { bool present = false, has = false; int type = 0; uint64_t lo = 0, hi = 0; std::string slo, shi; int32_t nulls = 0; };
-std::vector<uint8_t> stats_row_bytes(int32_t count, const std::vector<ColStat>& st) {
-  const int nf = 1 + 3 * (int)st.size();
-  const int64_t bits = ((nf + 63) / 64) * 8, fixed = bits + 8ll * nf;
-  std::vector<uint8_t> row((size_t)fixed, 0);
-  auto setnull = [&](int i) { row[i >> 3] |= (uint8_t)(1u << (i & 7)); };
+}  // namespace
+
+namespace {
+// entry f.. of a stats row: (lower, upper, nullCount) of one column, written over whatever the slots held; STRING bounds go
+// to the end of the variable-length region
+void put_entry(std::vector<uint8_t>& row, int64_t bits, int f, const ColStat& s) {
+  auto setnull = [&](int i, bool v) { if (v) row[i >> 3] |= (uint8_t)(1u << (i & 7)); else row[i >> 3] &= (uint8_t)~(1u << (i & 7)); };
   auto slot = [&](int i) { return row.data() + bits + 8ll * i; };
-  memcpy(slot(0), &count, 4);
-  for (size_t c = 0; c < st.size(); c++) {
-    const ColStat& s = st[c];
-    const int f = 1 + 3 * (int)c;
-    if (!s.present) { setnull(f); setnull(f + 1); setnull(f + 2); continue; }
-    memcpy(slot(f + 2), &s.nulls, 4);
-    if (!s.has) { setnull(f); setnull(f + 1); continue; }
-    for (int w = 0; w < 2; w++) {
-      if (s.type == SD_STRING) {
-        const std::string& v = w ? s.shi : s.slo;
-        const int64_t ol = ((int64_t)row.size() << 32) | (int64_t)v.size();
-        memcpy(slot(f + w), &ol, 8);
-        row.insert(row.end(), v.begin(), v.end());
-        while (row.size() % 8) row.push_back(0);
-      } else {
-        const uint64_t raw = w ? s.hi : s.lo;
-        switch (s.type) {
-          case SD_BOOLEAN: *slot(f + w) = raw != 0; break;
-          case SD_BYTE: memcpy(slot(f + w), &raw, 1); break;
-          case SD_SHORT: memcpy(slot(f + w), &raw, 2); break;
-          case SD_INT: case SD_DATE: memcpy(slot(f + w), &raw, 4); break;
-          case SD_FLOAT: { double d; memcpy(&d, &raw, 8); float fl = (float)d; memcpy(slot(f + w), &fl, 4); break; }
-          default: memcpy(slot(f + w), &raw, 8); break;
-        }
+  for (int k = 0; k < 3; k++) { memset(slot(f + k), 0, 8); setnull(f + k, !s.present); }
+  if (!s.present) return;
+  memcpy(slot(f + 2), &s.nulls, 4);
+  if (!s.has) { setnull(f, true); setnull(f + 1, true); return; }
+  for (int w = 0; w < 2; w++) {
+    if (s.type == SD_STRING) {
+      const std::string& v = w ? s.shi : s.slo;
+      const int64_t ol = ((int64_t)row.size() << 32) | (int64_t)v.size();
+      memcpy(slot(f + w), &ol, 8);
+      row.insert(row.end(), v.begin(), v.end());
+      while (row.size() % 8) row.push_back(0);
+    } else {
+      const uint64_t raw = w ? s.hi : s.lo;
+      switch (s.type) {
+        case SD_BOOLEAN: *slot(f + w) = raw != 0; break;
+        case SD_BYTE: memcpy(slot(f + w), &raw, 1); break;
+        case SD_SHORT: memcpy(slot(f + w), &raw, 2); break;
+        case SD_INT: case SD_DATE: memcpy(slot(f + w), &raw, 4); break;
+        case SD_FLOAT: { double d; memcpy(&d, &raw, 8); float fl = (float)d; memcpy(slot(f + w), &fl, 4); break; }
+        default: memcpy(slot(f + w), &raw, 8); break;
       }
     }
   }
+}
+int64_t stats_bits(int ncols) { return (int64_t)((1 + 3 * ncols + 63) / 64) * 8; }
+}  // namespace
+
+std::vector<uint8_t> stats_row_bytes(int32_t count, const std::vector<ColStat>& st) {
+  const int nf = 1 + 3 * (int)st.size();
+  const int64_t bits = stats_bits((int)st.size()), fixed = bits + 8ll * nf;
+  std::vector<uint8_t> row((size_t)fixed, 0);
+  memcpy(row.data() + bits, &count, 4);
+  for (size_t c = 0; c < st.size(); c++) put_entry(row, bits, 1 + 3 * (int)c, st[c]);
   return row;
 }
 
-}  // namespace
+void stats_row_replace(std::vector<uint8_t>& row, int ncols, int32_t count, const std::vector<std::pair<int, const ColStat*>>& entries) {
+  const int64_t bits = stats_bits(ncols);
+  if ((int64_t)row.size() < bits + 8ll * (1 + 3 * ncols)) return;   // not a stats row of ncols columns: left alone
+  memset(row.data() + bits, 0, 8);
+  memcpy(row.data() + bits, &count, 4);
+  for (auto& e : entries)
+    if (e.first < ncols) put_entry(row, bits, 1 + 3 * e.first, *e.second);
+}
+
+void enc_first_seen_dict(EncJob& j, std::vector<int2>& slot_first, const std::function<std::string(int slot, int first)>& value_of) {
+  std::sort(slot_first.begin(), slot_first.end(), [](const int2& a, const int2& b) { return a.y < b.y || (a.y == b.y && a.x < b.x); });
+  j.dict.clear();
+  j.slot_codes.clear();
+  for (size_t d = 0; d < slot_first.size(); d++) {
+    j.dict.push_back(value_of(slot_first[d].x, slot_first[d].y));
+    j.slot_codes.push_back(make_int2(slot_first[d].x, (int)d));
+  }
+}
+
+bool enc_queue_words(cudaStream_t st, const std::vector<EncJob*>& jobs, int* rc) {
+  bool any = false;
+  *rc = 0;
+  for (EncJob* j : jobs) {
+    if (j->fb[1] <= 0) continue;
+    j->words.resize((size_t)j->fb[1]);
+    const cudaError_t e = cudaMemcpyAsync(j->words.data(), j->d_words, (size_t)j->fb[1] * 8, cudaMemcpyDeviceToHost, st);
+    if (e != cudaSuccess) { *rc = set_error(SD_ERR_CUDA, "null words read-back failed: %s", cudaGetErrorString(e)); return any; }
+    any = true;
+  }
+  return any;
+}
+
+int enc_null_words_many(cudaStream_t st, const std::vector<EncJob*>& jobs, DevAllocFn alloc, void* ctx, PinnedArena& pin) {
+  std::vector<NullJob> nj;
+  int max_words = 0;
+  for (EncJob* j : jobs) {
+    if (!j->d_nulls || j->n <= 0) continue;
+    nj.push_back(NullJob{j->d_nulls, j->d_words, j->d_fb, j->n, 0});
+    max_words = std::max(max_words, (j->n + 63) / 64);
+  }
+  for (size_t at = 0; at < nj.size(); at += 65535) {   // gridDim.y limit
+    const size_t cnt = std::min<size_t>(65535, nj.size() - at);
+    uint8_t* h = pin.alloc(cnt * sizeof(NullJob));
+    uint8_t* d = alloc(ctx, cnt * sizeof(NullJob));
+    if (!h || !d) return SD_ERR_CUDA;
+    memcpy(h, nj.data() + at, cnt * sizeof(NullJob));
+    SD_CUDA(cudaMemcpyAsync(d, h, cnt * sizeof(NullJob), cudaMemcpyHostToDevice, st));
+    enc_null_words_many_kernel<<<dim3((unsigned)std::min(64, (max_words + 255) / 256), (unsigned)cnt), 256, 0, st>>>(reinterpret_cast<const NullJob*>(d));
+    SD_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+int enc_layout(sd_store* s, cudaStream_t st, PinnedArena& pin, EncJob& j, StoredCol& sc, ColStat& cs) {
+  const int nn = j.n - j.fb[0];
+  std::vector<uint8_t> pre;
+  int type_id = ENC_UNCOMPRESSED;
+  cs = ColStat();
+  if (j.type == SD_STRING) {
+    const int nd = (int)j.dict.size();
+    const bool big = nd > 32767;   // index Short.MaxValue switches to int32 indexes (enc/DictionaryEncoding.scala:313-318)
+    type_id = big ? ENC_BIG_DICTIONARY : ENC_DICTIONARY;
+    put32(pre, type_id); put32(pre, (int32_t)j.words.size() * 8);
+    pre.insert(pre.end(), reinterpret_cast<uint8_t*>(j.words.data()), reinterpret_cast<uint8_t*>(j.words.data()) + j.words.size() * 8);
+    put32(pre, nd);
+    for (const std::string& sv : j.dict) {
+      put32(pre, (int32_t)sv.size());
+      pre.insert(pre.end(), sv.begin(), sv.end());
+      if (!cs.has || sv < cs.slo) cs.slo = sv;      // std::string compares as unsigned bytes, shorter first on a common prefix
+      if (!cs.has || sv > cs.shi) cs.shi = sv;
+      cs.has = true;
+    }
+    j.body_len = (int64_t)nn * (big ? 4 : 2);
+  } else {
+    type_id = j.type == SD_BOOLEAN ? ENC_BOOLEAN_BITSET : ENC_UNCOMPRESSED;
+    put32(pre, type_id); put32(pre, (int32_t)j.words.size() * 8);
+    pre.insert(pre.end(), reinterpret_cast<uint8_t*>(j.words.data()), reinterpret_cast<uint8_t*>(j.words.data()) + j.words.size() * 8);
+    j.body_len = j.type == SD_BOOLEAN ? ((int64_t)(nn + 63) / 64) * 8 : (int64_t)nn * width_of(j.type);
+    cs.has = nn > 0;
+  }
+  int rc = store_register_encoded(s, pre.data(), (int64_t)pre.size(), (int64_t)pre.size() + j.body_len, j.type, j.nullable ? 1 : 0, j.n, sc);
+  if (rc) return rc;
+  uint8_t* h_pre = pin.alloc(pre.size());   // page-locked staging (stays valid until the stream has drained)
+  if (!h_pre) return SD_ERR_CUDA;
+  memcpy(h_pre, pre.data(), pre.size());
+  SD_CUDA(cudaMemcpyAsync(sc.dev_base, h_pre, pre.size(), cudaMemcpyHostToDevice, st));
+  j.d_body = sc.dev_base + pre.size();
+  if (j.type == SD_STRING && !j.slot_codes.empty()) {
+    uint8_t* h_pairs = pin.alloc(j.slot_codes.size() * 8);
+    if (!h_pairs) return SD_ERR_CUDA;
+    memcpy(h_pairs, j.slot_codes.data(), j.slot_codes.size() * 8);
+    SD_CUDA(cudaMemcpyAsync(j.d_slot_pairs, h_pairs, j.slot_codes.size() * 8, cudaMemcpyHostToDevice, st));
+    dict_codes_kernel<<<((int)j.slot_codes.size() + 255) / 256, 256, 0, st>>>(j.d_slot_pairs, (int)j.slot_codes.size(), j.d_slot_code);
+    SD_CUDA(cudaGetLastError());
+  }
+  if (j.type == SD_BOOLEAN && j.body_len) SD_CUDA(cudaMemsetAsync(j.d_body, 0, (size_t)j.body_len, st));
+  cs.present = true; cs.type = j.type; cs.nulls = j.fb[0];
+  return 0;
+}
+
+int enc_write(cudaStream_t st, DevAllocFn alloc, void* ctx, PinnedArena& pin, const std::vector<EncJob*>& jobs, const std::vector<ColStat*>& stats,
+              cudaEvent_t ev_begin, cudaEvent_t ev_end) {
+  if (jobs.empty()) return 0;
+  std::vector<EncCol> enc(jobs.size());
+  for (size_t k = 0; k < jobs.size(); k++) {
+    const EncJob& j = *jobs[k];
+    EncCol& e = enc[k];
+    memset(&e, 0, sizeof(e));
+    e.nulls = j.d_nulls; e.out = j.d_body; e.stat = j.d_stat; e.n = j.n;
+    if (j.type == SD_STRING) {
+      e.values = j.d_values;
+      e.kind = j.dict.size() > 32767 ? EK_STRCODE32 : EK_STRCODE16;
+      e.slot_code = j.d_slot_code;
+    } else {
+      e.values = j.d_values;
+      e.kind = kind_of(j.type);
+    }
+  }
+  uint8_t* d_enc = alloc(ctx, enc.size() * sizeof(EncCol) + 64);
+  uint8_t* h_enc = pin.alloc(enc.size() * sizeof(EncCol));
+  if (!d_enc || !h_enc) return SD_ERR_CUDA;
+  memcpy(h_enc, enc.data(), enc.size() * sizeof(EncCol));
+  SD_CUDA(cudaMemcpyAsync(d_enc, h_enc, enc.size() * sizeof(EncCol), cudaMemcpyHostToDevice, st));
+  if (ev_begin) SD_CUDA(cudaEventRecord(ev_begin, st));
+  enc_compact_kernel<<<(int)enc.size(), 1024, 0, st>>>(reinterpret_cast<const EncCol*>(d_enc));
+  SD_CUDA(cudaGetLastError());
+  if (ev_end) SD_CUDA(cudaEventRecord(ev_end, st));
+  std::vector<uint64_t> hst(jobs.size() * 3);
+  for (size_t k = 0; k < jobs.size(); k++) SD_CUDA(cudaMemcpyAsync(&hst[3 * k], jobs[k]->d_stat, 24, cudaMemcpyDeviceToHost, st));
+  SD_CUDA(cudaStreamSynchronize(st));
+  for (size_t k = 0; k < jobs.size(); k++) {
+    ColStat& cs = *stats[k];
+    if (jobs[k]->type != SD_STRING && cs.has) { cs.lo = hst[3 * k]; cs.hi = hst[3 * k + 1]; }
+    if ((int64_t)hst[3 * k + 2] != (int64_t)(jobs[k]->n - jobs[k]->fb[0])) return set_error(SD_ERR_CUDA, "encoder: non-null count mismatch in column %d", jobs[k]->table_col);
+  }
+  return 0;
+}
+
 }  // namespace sd
 
 extern "C" int sd_store_encode_batch(sd_store* s, int32_t num_rows, const sd_raw_column* cols, int32_t ncols, int32_t bucket_id, int64_t batch_id) {
@@ -250,6 +401,7 @@ extern "C" int sd_store_encode_batch(sd_store* s, int32_t num_rows, const sd_raw
   Arena tmp;
   tmp.device = s->device;
   tmp.slab_bytes = size_t(64) << 20;
+  const DevAllocFn tmp_alloc = [](void* a, size_t bytes) { return reinterpret_cast<Arena*>(a)->alloc(bytes, 16); };
   auto to_dev = [&](const void* src, size_t bytes, size_t align, uint8_t** out) -> int {
     uint8_t* d = tmp.alloc(bytes + 64, align);
     if (!d) return SD_ERR_CUDA;
@@ -259,173 +411,120 @@ extern "C" int sd_store_encode_batch(sd_store* s, int32_t num_rows, const sd_raw
     return 0;
   };
   struct Work {
-    int table_col; int type; bool nullable;
-    uint8_t *d_values = nullptr, *d_nulls = nullptr, *d_bytes = nullptr;
-    uint64_t* d_words = nullptr; int* d_fb = nullptr; uint64_t* d_stat = nullptr;
-    int *d_slots = nullptr, *d_count = nullptr; int32_t *d_slot_of_row = nullptr, *d_slot_code = nullptr; int2* d_pairs = nullptr; uint32_t cap = 0;
-    int fb[2] = {0, 0};
-    std::vector<uint64_t> words;
-    std::vector<uint8_t> prefix;
-    std::vector<std::string> dict;
-    bool big = false;
+    EncJob job;
+    uint8_t* d_bytes = nullptr;   // STRING: the values' bytes
+    int* d_slots = nullptr; int* d_count = nullptr; int2* d_pairs = nullptr; uint32_t cap = 0;
   };
   std::vector<Work> work;
   // ---- phase 1: raw values to the device; null words; distinct strings -------------------------------------------------
   for (int c = 0; c < ncols; c++) {
     if (!cols[c].values) continue;
     Work w;
-    w.table_col = c; w.type = s->schema[c].type; w.nullable = s->schema[c].nullable != 0;
-    if (cols[c].nulls && !w.nullable) return set_error(SD_ERR_INVALID, "column %d is NOT NULL but a null mask was given", c);
+    EncJob& j = w.job;
+    j.table_col = c; j.type = s->schema[c].type; j.nullable = s->schema[c].nullable != 0; j.n = n;
+    if (cols[c].nulls && !j.nullable) return set_error(SD_ERR_INVALID, "column %d is NOT NULL but a null mask was given", c);
     int rc = 0;
-    if (w.type == SD_STRING) {
+    uint8_t* d_values = nullptr;
+    if (j.type == SD_STRING) {
       const int32_t* offs = reinterpret_cast<const int32_t*>(cols[c].values);
       if (!cols[c].str_bytes && n > 0 && offs[n] > 0) return set_error(SD_ERR_INVALID, "column %d: STRING column without bytes", c);
-      rc = to_dev(offs, (size_t)(n + 1) * 4, 16, &w.d_values);
+      rc = to_dev(offs, (size_t)(n + 1) * 4, 16, &d_values);
       if (!rc) rc = to_dev(cols[c].str_bytes, n > 0 ? (size_t)offs[n] : 0, 16, &w.d_bytes);
     } else {
-      const int wd = width_of(w.type);
-      if (!wd) return set_error(SD_ERR_UNSUPPORTED, "column %d: type %d cannot be encoded", c, w.type);
-      rc = to_dev(cols[c].values, (size_t)n * wd, 16, &w.d_values);
+      const int wd = width_of(j.type);
+      if (!wd) return set_error(SD_ERR_UNSUPPORTED, "column %d: type %d cannot be encoded", c, j.type);
+      rc = to_dev(cols[c].values, (size_t)n * wd, 16, &d_values);
     }
     if (rc) return rc;
-    if (cols[c].nulls) { rc = to_dev(cols[c].nulls, (size_t)n, 16, &w.d_nulls); if (rc) return rc; }
-    w.d_stat = reinterpret_cast<uint64_t*>(tmp.alloc(64, 16));
-    w.d_fb = reinterpret_cast<int*>(tmp.alloc(64, 16));
-    if (!w.d_stat || !w.d_fb) return SD_ERR_CUDA;
-    SD_CUDA(cudaMemsetAsync(w.d_fb, 0, 64, st));
-    if (w.d_nulls && n > 0) {
-      const int nw = (n + 63) / 64;
-      w.d_words = reinterpret_cast<uint64_t*>(tmp.alloc((size_t)nw * 8 + 64, 16));
-      if (!w.d_words) return SD_ERR_CUDA;
-      enc_null_words_kernel<<<(nw + 255) / 256, 256, 0, st>>>(w.d_nulls, n, w.d_words, w.d_fb);
-      SD_CUDA(cudaGetLastError());
+    j.d_values = d_values;
+    if (cols[c].nulls) {
+      uint8_t* d_nulls = nullptr;
+      rc = to_dev(cols[c].nulls, (size_t)n, 16, &d_nulls);
+      if (rc) return rc;
+      j.d_nulls = d_nulls;
     }
-    if (w.type == SD_STRING && n > 0) {
+    j.d_stat = reinterpret_cast<uint64_t*>(tmp.alloc(64, 16));
+    j.d_fb = reinterpret_cast<int*>(tmp.alloc(64, 16));
+    if (!j.d_stat || !j.d_fb) return SD_ERR_CUDA;
+    SD_CUDA(cudaMemsetAsync(j.d_fb, 0, 64, st));
+    if (j.d_nulls && n > 0) {
+      const int nw = (n + 63) / 64;
+      j.d_words = reinterpret_cast<uint64_t*>(tmp.alloc((size_t)nw * 8 + 64, 16));
+      if (!j.d_words) return SD_ERR_CUDA;
+    }
+    if (j.type == SD_STRING && n > 0) {
       w.cap = 1024;
       while (w.cap < 2u * (uint32_t)n) w.cap <<= 1;
       w.d_slots = reinterpret_cast<int*>(tmp.alloc((size_t)w.cap * 4, 16));
-      w.d_slot_code = reinterpret_cast<int32_t*>(tmp.alloc((size_t)w.cap * 4, 16));
-      w.d_slot_of_row = reinterpret_cast<int32_t*>(tmp.alloc((size_t)n * 4 + 64, 16));
+      j.d_slot_code = reinterpret_cast<int32_t*>(tmp.alloc((size_t)w.cap * 4, 16));
+      int32_t* d_slot_of_row = reinterpret_cast<int32_t*>(tmp.alloc((size_t)n * 4 + 64, 16));
       w.d_pairs = reinterpret_cast<int2*>(tmp.alloc((size_t)n * 8 + 64, 16));
       w.d_count = reinterpret_cast<int*>(tmp.alloc(64, 16));
-      if (!w.d_slots || !w.d_slot_code || !w.d_slot_of_row || !w.d_pairs || !w.d_count) return SD_ERR_CUDA;
+      if (!w.d_slots || !j.d_slot_code || !d_slot_of_row || !w.d_pairs || !w.d_count) return SD_ERR_CUDA;
       SD_CUDA(cudaMemsetAsync(w.d_slots, 0xff, (size_t)w.cap * 4, st));
       SD_CUDA(cudaMemsetAsync(w.d_count, 0, 4, st));
-      dict_insert_kernel<<<592, 256, 0, st>>>(reinterpret_cast<const int32_t*>(w.d_values), w.d_bytes, w.d_nulls, n, w.d_slots, w.cap - 1, w.d_slot_of_row);
+      dict_insert_kernel<<<592, 256, 0, st>>>(reinterpret_cast<const int32_t*>(d_values), w.d_bytes, j.d_nulls, n, w.d_slots, w.cap - 1, d_slot_of_row);
       SD_CUDA(cudaGetLastError());
       dict_collect_kernel<<<592, 256, 0, st>>>(w.d_slots, w.cap, w.d_pairs, w.d_count);
       SD_CUDA(cudaGetLastError());
+      j.d_values = reinterpret_cast<const uint8_t*>(d_slot_of_row);   // the encoder reads the slot of every row
+      j.d_slot_pairs = w.d_pairs;
     }
     work.push_back(std::move(w));
+  }
+  std::vector<EncJob*> jobs;
+  for (Work& w : work) jobs.push_back(&w.job);
+  {
+    int rc = enc_null_words_many(st, jobs, tmp_alloc, &tmp, s->enc_host);
+    if (rc) return rc;
   }
   // ---- feedback: null counts / trimmed word counts / null words, distinct strings ----------------------------------------
   std::vector<std::vector<int2>> pairs(work.size());
   std::vector<int> ndistinct(work.size(), 0);
   for (size_t k = 0; k < work.size(); k++) {
     Work& w = work[k];
-    SD_CUDA(cudaMemcpyAsync(w.fb, w.d_fb, 8, cudaMemcpyDeviceToHost, st));
+    SD_CUDA(cudaMemcpyAsync(w.job.fb, w.job.d_fb, 8, cudaMemcpyDeviceToHost, st));
     if (w.d_count) SD_CUDA(cudaMemcpyAsync(&ndistinct[k], w.d_count, 4, cudaMemcpyDeviceToHost, st));
   }
   SD_CUDA(cudaStreamSynchronize(st));
+  {
+    int rc = 0;
+    enc_queue_words(st, jobs, &rc);
+    if (rc) return rc;
+  }
   for (size_t k = 0; k < work.size(); k++) {
-    Work& w = work[k];
-    if (w.fb[1] > 0) { w.words.resize((size_t)w.fb[1]); SD_CUDA(cudaMemcpyAsync(w.words.data(), w.d_words, (size_t)w.fb[1] * 8, cudaMemcpyDeviceToHost, st)); }
-    if (ndistinct[k] > 0) { pairs[k].resize((size_t)ndistinct[k]); SD_CUDA(cudaMemcpyAsync(pairs[k].data(), w.d_pairs, (size_t)ndistinct[k] * 8, cudaMemcpyDeviceToHost, st)); }
+    if (ndistinct[k] > 0) { pairs[k].resize((size_t)ndistinct[k]); SD_CUDA(cudaMemcpyAsync(pairs[k].data(), work[k].d_pairs, (size_t)ndistinct[k] * 8, cudaMemcpyDeviceToHost, st)); }
   }
   SD_CUDA(cudaStreamSynchronize(st));
-  // ---- layout on the host; registration in the store; phase 2 descriptors ------------------------------------------------
+  // dictionary in first-seen order: the distinct strings by the earliest row that holds them
+  for (size_t k = 0; k < work.size(); k++) {
+    EncJob& j = work[k].job;
+    if (j.type != SD_STRING) continue;
+    const int32_t* offs = reinterpret_cast<const int32_t*>(cols[j.table_col].values);
+    const uint8_t* bytes = cols[j.table_col].str_bytes;
+    enc_first_seen_dict(j, pairs[k], [&](int, int row) {
+      return std::string(reinterpret_cast<const char*>(bytes + offs[row]), (size_t)(offs[row + 1] - offs[row]));
+    });
+  }
+  // ---- layout on the host; registration in the store; phase 2 ----------------------------------------------------------
   std::unique_ptr<StoredBatch> sb(new StoredBatch());
   sb->num_rows = n; sb->bucket_id = bucket_id; sb->batch_id = batch_id;
   sb->cols.resize(s->schema.size());
-  std::vector<EncCol> enc(work.size());
   std::vector<ColStat> stats(s->schema.size());
+  std::vector<ColStat*> job_stats;
   std::unique_lock<std::mutex> store_lock(s->mu);   // phase 2: arena placement + the small side uploads of upload_column
-  for (size_t k = 0; k < work.size(); k++) {
-    Work& w = work[k];
-    const int nn = n - w.fb[0];
-    std::vector<uint8_t>& pre = w.prefix;
-    int type_id = ENC_UNCOMPRESSED;
-    int64_t body_len = 0;
-    if (w.type == SD_STRING) {
-      // dictionary in first-seen order: sort the distinct strings by the earliest row that holds them
-      std::sort(pairs[k].begin(), pairs[k].end(), [](const int2& a, const int2& b) { return a.y < b.y; });
-      const int32_t* offs = reinterpret_cast<const int32_t*>(cols[w.table_col].values);
-      const int nd = (int)pairs[k].size();
-      w.big = nd > 32767;   // index Short.MaxValue switches to int32 indexes (enc/DictionaryEncoding.scala:313-318)
-      type_id = w.big ? ENC_BIG_DICTIONARY : ENC_DICTIONARY;
-      put32(pre, type_id); put32(pre, (int32_t)w.words.size() * 8);
-      pre.insert(pre.end(), reinterpret_cast<uint8_t*>(w.words.data()), reinterpret_cast<uint8_t*>(w.words.data()) + w.words.size() * 8);
-      put32(pre, nd);
-      ColStat& cs = stats[w.table_col];
-      for (int j = 0; j < nd; j++) {
-        const int row = pairs[k][j].y;
-        const int32_t l = offs[row + 1] - offs[row];
-        put32(pre, l);
-        pre.insert(pre.end(), cols[w.table_col].str_bytes + offs[row], cols[w.table_col].str_bytes + offs[row] + l);
-        std::string sv(reinterpret_cast<const char*>(cols[w.table_col].str_bytes + offs[row]), (size_t)l);
-        if (!cs.has || sv < cs.slo) cs.slo = sv;      // std::string compares as unsigned bytes, shorter first on a common prefix
-        if (!cs.has || sv > cs.shi) cs.shi = sv;
-        cs.has = true;
-        pairs[k][j].y = j;                            // slot -> code
-      }
-      body_len = (int64_t)nn * (w.big ? 4 : 2);
-    } else {
-      type_id = w.type == SD_BOOLEAN ? ENC_BOOLEAN_BITSET : ENC_UNCOMPRESSED;
-      put32(pre, type_id); put32(pre, (int32_t)w.words.size() * 8);
-      pre.insert(pre.end(), reinterpret_cast<uint8_t*>(w.words.data()), reinterpret_cast<uint8_t*>(w.words.data()) + w.words.size() * 8);
-      body_len = w.type == SD_BOOLEAN ? ((int64_t)(nn + 63) / 64) * 8 : (int64_t)nn * width_of(w.type);
-    }
-    StoredCol& sc = sb->cols[w.table_col];
-    int rc = store_register_encoded(s, pre.data(), (int64_t)pre.size(), (int64_t)pre.size() + body_len, w.type, w.nullable ? 1 : 0, n, sc);
+  for (Work& w : work) {
+    int rc = enc_layout(s, st, s->enc_host, w.job, sb->cols[w.job.table_col], stats[w.job.table_col]);
     if (rc) return rc;
-    uint8_t* h_pre = s->enc_host.alloc(pre.size());   // page-locked staging (stays valid until the stream has drained)
-    if (!h_pre) return SD_ERR_CUDA;
-    memcpy(h_pre, pre.data(), pre.size());
-    SD_CUDA(cudaMemcpyAsync(sc.dev_base, h_pre, pre.size(), cudaMemcpyHostToDevice, st));
-    EncCol& e = enc[k];
-    memset(&e, 0, sizeof(e));
-    e.nulls = w.d_nulls; e.out = sc.dev_base + pre.size(); e.stat = w.d_stat; e.n = n;
-    if (w.type == SD_STRING) {
-      e.values = reinterpret_cast<const uint8_t*>(w.d_slot_of_row);
-      e.kind = w.big ? EK_STRCODE32 : EK_STRCODE16;
-      if (!pairs[k].empty()) {
-        uint8_t* h_pairs = s->enc_host.alloc(pairs[k].size() * 8);
-        if (!h_pairs) return SD_ERR_CUDA;
-        memcpy(h_pairs, pairs[k].data(), pairs[k].size() * 8);
-        SD_CUDA(cudaMemcpyAsync(w.d_pairs, h_pairs, pairs[k].size() * 8, cudaMemcpyHostToDevice, st));
-        dict_codes_kernel<<<((int)pairs[k].size() + 255) / 256, 256, 0, st>>>(w.d_pairs, (int)pairs[k].size(), w.d_slot_code);
-        SD_CUDA(cudaGetLastError());
-      }
-      e.slot_code = w.d_slot_code;
-    } else {
-      e.values = w.d_values;
-      e.kind = kind_of(w.type);
-      if (w.type == SD_BOOLEAN && body_len) SD_CUDA(cudaMemsetAsync(e.out, 0, (size_t)body_len, st));
-    }
-    ColStat& cs = stats[w.table_col];
-    cs.present = true; cs.type = w.type; cs.nulls = w.fb[0];
-    if (w.type != SD_STRING) cs.has = nn > 0;
+    job_stats.push_back(&stats[w.job.table_col]);
   }
   // the side uploads (null words, prefixes of "nulls before") went over the store's copy stream: order the encoder after them
   SD_CUDA(cudaEventRecord(s->enc_event, s->copy_stream));
   SD_CUDA(cudaStreamWaitEvent(st, s->enc_event, 0));
   store_lock.unlock();
-  if (!work.empty()) {
-    uint8_t* d_enc = tmp.alloc(enc.size() * sizeof(EncCol) + 64, 16);
-    uint8_t* h_enc = s->enc_host.alloc(enc.size() * sizeof(EncCol));
-    if (!d_enc || !h_enc) return SD_ERR_CUDA;
-    memcpy(h_enc, enc.data(), enc.size() * sizeof(EncCol));
-    SD_CUDA(cudaMemcpyAsync(d_enc, h_enc, enc.size() * sizeof(EncCol), cudaMemcpyHostToDevice, st));
-    enc_compact_kernel<<<(int)enc.size(), 1024, 0, st>>>(reinterpret_cast<const EncCol*>(d_enc));
-    SD_CUDA(cudaGetLastError());
-    std::vector<uint64_t> hst(work.size() * 3);
-    for (size_t k = 0; k < work.size(); k++) SD_CUDA(cudaMemcpyAsync(&hst[3 * k], work[k].d_stat, 24, cudaMemcpyDeviceToHost, st));
-    SD_CUDA(cudaStreamSynchronize(st));
-    for (size_t k = 0; k < work.size(); k++) {
-      ColStat& cs = stats[work[k].table_col];
-      if (work[k].type != SD_STRING && cs.has) { cs.lo = hst[3 * k]; cs.hi = hst[3 * k + 1]; }
-      if ((int64_t)hst[3 * k + 2] != (int64_t)(n - work[k].fb[0])) return set_error(SD_ERR_CUDA, "encoder: non-null count mismatch in column %d", work[k].table_col);
-    }
+  {
+    int rc = enc_write(st, tmp_alloc, &tmp, s->enc_host, jobs, job_stats);
+    if (rc) return rc;
   }
   sb->stats = stats_row_bytes(n, stats);
   sb->stats_ncols = (int32_t)s->schema.size();

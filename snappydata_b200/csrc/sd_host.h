@@ -6,6 +6,7 @@
 
 #include <atomic>
 #include <cstdint>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -180,8 +181,8 @@ struct StoredBatch {
 
 struct sd_store {
   // ingest (sd_store_put_batch) may run concurrently with scans: `mu` guards batches / arena / version / the LZ4 queues.  A scan
-  // works on the SNAPSHOT of batch pointers it takes under the lock when it starts (batches are never removed or moved
-  // while the store lives; a batch becomes visible only after its bytes have reached the device).
+  // works on the SNAPSHOT of batch pointers it takes under the lock when it starts (a batch becomes visible only after its
+  // bytes have reached the device; a batch replaced or removed by UPDATE / DELETE / compaction stays alive in `retired`).
   std::mutex mu;
   int device = 0;
   std::vector<sd_column> schema;
@@ -193,8 +194,9 @@ struct sd_store {
   int next_stream = 0;
   cudaEvent_t extra_done[4] = {nullptr, nullptr, nullptr, nullptr};
   std::vector<std::unique_ptr<sd::StoredBatch>> batches;
-  // UPDATE / DELETE replace a batch by a new version at the same index; the old one stays alive here until the store is
-  // destroyed (scans hold raw pointers into their snapshot).  `mutate_mu` serialises the statements on this store.
+  // UPDATE / DELETE / compaction replace a batch by a new version at the same index (compaction also drops fully deleted
+  // batches); the old one stays alive here until the store is destroyed (scans hold raw pointers into their snapshot).
+  // `mutate_mu` serialises the statements and compactions on this store.
   std::vector<std::unique_ptr<sd::StoredBatch>> retired;
   std::mutex mutate_mu;
   int64_t version = 0;
@@ -247,6 +249,72 @@ int mutation_scan(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nb
                   MutationScan* out);
 // the analysed plan of a handle (sd_engine.cu)
 const PlanSpec& plan_spec(const sd_plan* p);
+
+// device scratch of one statement / compaction round, stream-ordered (cudaMallocAsync / cudaFreeAsync: no device-wide
+// synchronisation, so queries running on other streams are not stalled by its allocations), released when it ends
+struct DevScratch {
+  cudaStream_t st = nullptr;
+  std::vector<void*> ptrs;
+  template <class T> int get(T** out, size_t bytes) {
+    void* p = nullptr;
+    SD_CUDA(cudaMallocAsync(&p, bytes ? bytes : 16, st));
+    ptrs.push_back(p);
+    *out = reinterpret_cast<T*>(p);
+    return 0;
+  }
+  ~DevScratch() { for (void* p : ptrs) cudaFreeAsync(p, st); }
+};
+
+// install new batch versions and drop batches, all under ONE hold of the store's lock (a scan's snapshot sees every change
+// or none): fresh[i].second replaces fresh[i].first at its index, `remove` leaves the store; the replaced and removed
+// versions move to `retired` (scans of an older snapshot may still read them).  SD_ERR_STATE, nothing changed, when one
+// of the named batches is no longer in the store (sd_store.cu)
+typedef std::vector<std::pair<const StoredBatch*, std::unique_ptr<StoredBatch>>> FreshBatches;
+int store_install(sd_store* s, FreshBatches& fresh, const std::vector<const StoredBatch*>& remove, const char* what);
+
+// ---- the device encoder (sd_encode.cu): raw column values resident on the device -> encoded buffers in the store ---------
+// Shared by ingest (sd_store_encode_batch, one batch) and compaction (sd_compact.cu, the columns of many batches at once).
+// Per column: enc_null_words_many (null words + null count, one launch for all), read back fb / words (enc_queue_words), enc_layout under the store's lock (header,
+// trimmed null words, dictionary in first-seen order; arena placement through store_register_encoded), then ONE
+// enc_write launch for every column of the call (compacted values / bit set / dictionary indexes, min / max).
+struct ColStat { bool present = false, has = false; int type = 0; uint64_t lo = 0, hi = 0; std::string slo, shi; int32_t nulls = 0; };
+// stats UnsafeRow [count:int][(lower, upper, nullCount:int) per table column] (enc/ColumnEncoding.scala:1015-1036)
+std::vector<uint8_t> stats_row_bytes(int32_t count, const std::vector<ColStat>& st);
+// a stats row of ncols columns with a new count and the given columns' entries replaced; every other entry keeps its bytes
+// (replaced STRING bounds are appended to the variable-length region)
+void stats_row_replace(std::vector<uint8_t>& row, int ncols, int32_t count, const std::vector<std::pair<int, const ColStat*>>& entries);
+struct EncJob {
+  int table_col = 0, type = 0, n = 0;
+  bool nullable = false;
+  const uint8_t* d_values = nullptr;   // n values of the type's width (BOOLEAN: one byte); STRING: int32 "slot" per row
+  const uint8_t* d_nulls = nullptr;    // n null flags (one byte, non-zero = NULL) or nullptr
+  int32_t* d_slot_code = nullptr;      // STRING: slot -> dictionary index, filled by enc_layout from slot_codes
+  int2* d_slot_pairs = nullptr;        // STRING: device room for slot_codes
+  std::vector<std::string> dict;       // STRING: the distinct values in first-seen order
+  std::vector<int2> slot_codes;        // STRING: (slot, dictionary index) of every distinct value
+  // set by the encoder
+  uint64_t* d_words = nullptr;         // null words (room for ceil(n / 64))
+  int* d_fb = nullptr;                 // [0] nulls [1] last non-zero null word + 1 (zeroed by the caller)
+  uint64_t* d_stat = nullptr;          // [0] lower [1] upper [2] non-null count
+  int fb[2] = {0, 0};
+  std::vector<uint64_t> words;         // the trimmed null words, read back
+  uint8_t* d_body = nullptr;           // where enc_write puts the body
+  int64_t body_len = 0;
+};
+typedef uint8_t* (*DevAllocFn)(void* ctx, size_t bytes);   // 16-byte aligned device scratch, nullptr on failure (error set)
+// the null words of every job with nulls, in one launch (d_words / d_fb must be set, d_fb zeroed)
+int enc_null_words_many(cudaStream_t st, const std::vector<EncJob*>& jobs, DevAllocFn alloc, void* ctx, PinnedArena& pin);
+// after fb has been read back: queue the read-back of the trimmed null words of the jobs that hold NULLs (true: some were
+// queued; the caller synchronises); *rc: error
+bool enc_queue_words(cudaStream_t st, const std::vector<EncJob*>& jobs, int* rc);
+// STRING: the dictionary in first-seen order from (slot, first position) of every distinct value -> j.dict, j.slot_codes
+void enc_first_seen_dict(EncJob& j, std::vector<int2>& slot_first, const std::function<std::string(int slot, int first)>& value_of);
+// lay one column out in the arena (caller holds s->mu): registers `sc`, queues the prefix upload, sets d_body and the stats
+int enc_layout(sd_store* s, cudaStream_t st, PinnedArena& pin, EncJob& j, StoredCol& sc, ColStat& cs);
+// write every job's body in one launch and finish the stats (the caller has ordered `st` after the side uploads)
+// (ev_begin / ev_end, when given, are recorded around the launch)
+int enc_write(cudaStream_t st, DevAllocFn alloc, void* ctx, PinnedArena& pin, const std::vector<EncJob*>& jobs,
+              const std::vector<ColStat*>& stats, cudaEvent_t ev_begin = nullptr, cudaEvent_t ev_end = nullptr);
 }
 
 #endif

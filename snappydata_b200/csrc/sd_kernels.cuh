@@ -24,6 +24,8 @@
 //     CTA, then by the last CTA in fixed order.
 //
 // Self-contained: includes only sd_device.h so NVRTC can compile it from an in-memory string.
+// Included by more than one translation unit (the plan kernels, sd_compact.cu): out-of-line helpers that are not templates
+// have internal linkage.
 #ifndef SD_KERNELS_CUH
 #define SD_KERNELS_CUH
 
@@ -69,32 +71,32 @@ __device__ __forceinline__ int tv_not(int a) { return a == 2 ? 2 : 1 - a; }
 __device__ __forceinline__ int rec_len(const uint8_t* rec) {
   return (int)((uint32_t)rec[0] | ((uint32_t)rec[1] << 8) | ((uint32_t)rec[2] << 16) | ((uint32_t)rec[3] << 24));
 }
-__device__ __noinline__ int str_cmp_rec(const uint8_t* rec, const uint8_t* lit, int llen) {
+static __device__ __noinline__ int str_cmp_rec(const uint8_t* rec, const uint8_t* lit, int llen) {
   const int n = rec_len(rec);
   const uint8_t* s = rec + 4;
   const int m = n < llen ? n : llen;
   for (int i = 0; i < m; i++) { const int d = (int)s[i] - (int)lit[i]; if (d) return d; }
   return n - llen;
 }
-__device__ __noinline__ bool str_starts_rec(const uint8_t* rec, const uint8_t* lit, int llen) {
+static __device__ __noinline__ bool str_starts_rec(const uint8_t* rec, const uint8_t* lit, int llen) {
   if (rec_len(rec) < llen) return false;
   const uint8_t* s = rec + 4;
   for (int i = 0; i < llen; i++) if (s[i] != lit[i]) return false;
   return true;
 }
-__device__ __noinline__ bool str_eq_recs(const uint8_t* a, const uint8_t* b) {
+static __device__ __noinline__ bool str_eq_recs(const uint8_t* a, const uint8_t* b) {
   if (a == b) return true;
   const int n = rec_len(a);
   if (n != rec_len(b)) return false;
   for (int i = 0; i < n; i++) if (a[4 + i] != b[4 + i]) return false;
   return true;
 }
-__device__ __noinline__ int str_cmp_recs(const uint8_t* a, const uint8_t* b) {   // UTF8String.compareTo on two records
+static __device__ __noinline__ int str_cmp_recs(const uint8_t* a, const uint8_t* b) {   // UTF8String.compareTo on two records
   const int na = rec_len(a), nb = rec_len(b), m = na < nb ? na : nb;
   for (int i = 0; i < m; i++) { const int d = (int)a[4 + i] - (int)b[4 + i]; if (d) return d; }
   return na - nb;
 }
-__device__ __noinline__ uint64_t str_hash_rec(const uint8_t* rec) {   // FNV-1a over the bytes
+static __device__ __noinline__ uint64_t str_hash_rec(const uint8_t* rec) {   // FNV-1a over the bytes
   const int n = rec_len(rec);
   uint64_t h = 1469598103934665603ull;
   for (int i = 0; i < n; i++) { h ^= rec[4 + i]; h *= 1099511628211ull; }
@@ -462,7 +464,7 @@ __device__ __forceinline__ uint64_t warp_segment_mask(const int32_t* pos, int n,
   }
   return mask;
 }
-__device__ __noinline__ int warp_cursor_init(const int32_t* pos, int n, int32_t a) { return lower_bound_i32(pos, 0, n, a); }
+static __device__ __noinline__ int warp_cursor_init(const int32_t* pos, int n, int32_t a) { return lower_bound_i32(pos, 0, n, a); }
 
 // overlay of one column, per warp: rows whose position is in the depth-0 delta take that value, else the depth-1 delta's
 // (enc/UpdatedColumnDecoder.scala:95-104)
@@ -570,7 +572,7 @@ __device__ __forceinline__ void warp_find_range(const int32_t* positions, int n,
   *out_hi = hi;
 }
 // one copy for all columns and plans (out of line: see decode_value_slow)
-__device__ __noinline__ void find_delta_ranges(const DevDelta* d0, const DevDelta* d1, int32_t ts, int32_t te, bool first_tile, int32_t* drange, int lane) {
+static __device__ __noinline__ void find_delta_ranges(const DevDelta* d0, const DevDelta* d1, int32_t ts, int32_t te, bool first_tile, int32_t* drange, int lane) {
 #pragma unroll
   for (int dd = 0; dd < 2; dd++) {
     const DevDelta* d = dd == 0 ? d0 : d1;
@@ -581,7 +583,7 @@ __device__ __noinline__ void find_delta_ranges(const DevDelta* d0, const DevDelt
     if (lane == 0) { drange[2 * dd] = lo; drange[2 * dd + 1] = hi; }
   }
 }
-__device__ __noinline__ void find_delete_range(const int32_t* deletes, int n, int32_t ts, int32_t te, bool first_tile, int32_t* delrange, int lane) {
+static __device__ __noinline__ void find_delete_range(const int32_t* deletes, int n, int32_t ts, int32_t te, bool first_tile, int32_t* delrange, int lane) {
   int lo, hi;
   const int first = first_tile ? -1 : delrange[1];
   warp_find_range(deletes, n, ts, te, first, lane, &lo, &hi);

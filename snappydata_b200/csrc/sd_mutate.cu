@@ -261,21 +261,6 @@ int width_of_type(int t) {
   return 0;
 }
 
-// device scratch of one statement, stream-ordered (cudaMallocAsync / cudaFreeAsync: no device-wide synchronisation, so queries
-// running on other streams are not stalled by a statement's allocations), released when the statement ends
-struct DevScratch {
-  cudaStream_t st = nullptr;
-  std::vector<void*> ptrs;
-  template <class T> int get(T** out, size_t bytes) {
-    void* p = nullptr;
-    SD_CUDA(cudaMallocAsync(&p, bytes ? bytes : 16, st));
-    ptrs.push_back(p);
-    *out = reinterpret_cast<T*>(p);
-    return 0;
-  }
-  ~DevScratch() { for (void* p : ptrs) cudaFreeAsync(p, st); }
-};
-
 // ---- ColumnDelta.mergeStats (ColumnDelta.scala:134-222) on the host copy of a batch's stats row --------------------------
 uint64_t key_to_raw(int type, uint64_t k) {   // inverse of value_key
   if (type != SD_FLOAT && type != SD_DOUBLE) return k ^ 0x8000000000000000ull;
@@ -484,7 +469,7 @@ int run_statement(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nb
   SD_CUDA(cudaStreamSynchronize(st));
   const auto t_inst = std::chrono::steady_clock::now();
   // ---- new batch versions -------------------------------------------------------------------------------------------------
-  std::vector<std::pair<const StoredBatch*, std::unique_ptr<StoredBatch>>> fresh;
+  FreshBatches fresh;
   for (int b = 0; b < nb; b++) {
     bool touched = false;
     for (int t = 0; t < T; t++) touched = touched || counts[(size_t)b * T + t].n_new > 0;
@@ -517,21 +502,8 @@ int run_statement(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nb
     }
     fresh.emplace_back(&old, std::move(nbp));
   }
-  {   // install: every new version of the statement under one hold of the store's lock
-    std::lock_guard<std::mutex> lock(s->mu);
-    std::unordered_map<const StoredBatch*, size_t> where;
-    for (size_t i = 0; i < s->batches.size(); i++) where.emplace(s->batches[i].get(), i);
-    for (auto& f : fresh) {
-      auto it = where.find(f.first);
-      if (it == where.end()) return set_error(SD_ERR_STATE, "%s: a batch of the statement's snapshot left the store", what);
-    }
-    for (auto& f : fresh) {
-      const size_t i = where[f.first];
-      s->retired.push_back(std::move(s->batches[i]));
-      s->batches[i] = std::move(f.second);
-    }
-    s->version++;
-  }
+  // install: every new version of the statement under one hold of the store's lock
+  if ((rc = store_install(s, fresh, {}, what))) return rc;
   *rows_out = ms.count;
   const auto t1 = std::chrono::steady_clock::now();
   float a = 0, bms = 0;

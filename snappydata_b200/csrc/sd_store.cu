@@ -611,6 +611,33 @@ static int upload_delta(sd_store* s, const uint8_t* buf, int64_t len, int type, 
   return 0;
 }
 
+int store_install(sd_store* s, FreshBatches& fresh, const std::vector<const StoredBatch*>& remove, const char* what) {
+  std::lock_guard<std::mutex> lock(s->mu);
+  std::unordered_map<const StoredBatch*, size_t> where;
+  for (size_t i = 0; i < s->batches.size(); i++) where.emplace(s->batches[i].get(), i);
+  for (auto& f : fresh)
+    if (!where.count(f.first)) return set_error(SD_ERR_STATE, "%s: a batch of the snapshot left the store", what);
+  for (const StoredBatch* r : remove)
+    if (!where.count(r)) return set_error(SD_ERR_STATE, "%s: a batch of the snapshot left the store", what);
+  for (auto& f : fresh) {
+    const size_t i = where[f.first];
+    s->retired.push_back(std::move(s->batches[i]));
+    s->batches[i] = std::move(f.second);
+  }
+  if (!remove.empty()) {
+    std::vector<bool> drop(s->batches.size(), false);
+    for (const StoredBatch* r : remove) drop[where[r]] = true;
+    size_t k = 0;
+    for (size_t i = 0; i < s->batches.size(); i++) {
+      if (drop[i]) s->retired.push_back(std::move(s->batches[i]));
+      else s->batches[k++] = std::move(s->batches[i]);
+    }
+    s->batches.resize(k);
+  }
+  s->version++;
+  return 0;
+}
+
 int store_register_encoded(sd_store* s, const uint8_t* prefix, int64_t prefix_len, int64_t total_len, int type, int nullable,
                            int num_rows, StoredCol& c) {
   if (total_len < prefix_len) return set_error(SD_ERR_INVALID, "encoded column shorter than its prefix");

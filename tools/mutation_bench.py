@@ -6,9 +6,13 @@ For each scale factor and selectivity: a fresh device-generated store (Q1's seve
 with k ship dates of 2526 chosen for the selectivity.  Per statement: the host clock around the synchronous call, the scan
 kernels' time and algorithmic GB/s (the plan's algorithmicBytes over the scan time, against the 3.35 TB/s data sheet), the sort
 and merge kernel times, the host install time (sdx_last_mutation_timing), and the Q1 kernel time over the store before and after
-(the cost of the overlay path).  One JSON line per statement on stdout.
+(the cost of the overlay path).  After each statement the store is compacted (sd_store_compact, every dirty batch): the
+call's host clock, its device phases (materialise + encode, sdx_last_compaction_timing), the bytes it read and wrote, their
+algorithmic GB/s over the device time, sd_store_bytes before and after, the store's compressible and total slab bytes
+afterwards (sdx_store_memory_info), and the Q1 kernel time over the compacted store.
+One JSON line per statement on stdout.
 
-    python tools/mutation_bench.py --sf 10 100 --sel 0.001 0.01 0.1
+    python tools/mutation_bench.py --sf 10 100 --sel 0.001 0.01 0.1 [--run 2]
 """
 import argparse
 import json
@@ -42,6 +46,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sf", type=int, nargs="+", default=[10, 100])
     ap.add_argument("--sel", type=float, nargs="+", default=[0.001, 0.01, 0.1])
+    ap.add_argument("--run", type=int, default=None, help="label written into every line (repeated runs in one file)")
     a = ap.parse_args()
     api = capi.product_api()
     api.check(api.init(0))
@@ -71,13 +76,29 @@ def main():
                 algo = p.metrics()["algorithmicBytes"]
                 p.close()
                 q1_after = q1_kernel_ms(api, store)
-                print(json.dumps({"sf": sf, "rows": total, "statement": kind, "selectivity": sel, "ship_dates": k, "rows_changed": rows,
+                bytes_before = store.nbytes()
+                t = time.perf_counter()
+                cc = store.compact(0.0)
+                c_wall = (time.perf_counter() - t) * 1e3
+                ct = capi.last_compaction_timing(api)
+                dev_ms = ct["materialise_ms"] + ct["encode_ms"]
+                q1_compacted = q1_kernel_ms(api, store)
+                print(json.dumps(({"run": a.run} if a.run is not None else {}) | {"sf": sf, "rows": total, "statement": kind, "selectivity": sel, "ship_dates": k, "rows_changed": rows,
                                   "fraction": rows / total, "statement_ms": round(wall, 3), "scan_ms": round(tm["scan_ms"], 3),
                                   "scan_algorithmic_bytes": algo, "scan_gbps": round(algo / (tm["scan_ms"] * 1e6), 1),
                                   "scan_frac_of_3350": round(algo / (tm["scan_ms"] * 1e6) / 3350.0, 3),
                                   "sort_ms": round(tm["sort_ms"], 3), "merge_ms": round(tm["merge_ms"], 3),
                                   "install_ms": round(tm["install_ms"], 3), "q1_kernel_ms_unmutated": round(q1_before, 3),
-                                  "q1_kernel_ms_after": round(q1_after, 3)}), flush=True)
+                                  "q1_kernel_ms_after": round(q1_after, 3),
+                                  "compaction_ms": round(c_wall, 3), "compaction_device_ms": round(dev_ms, 3),
+                                  "compaction_materialise_ms": round(ct["materialise_ms"], 3), "compaction_encode_ms": round(ct["encode_ms"], 3),
+                                  "compaction_host_ms": round(ct["host_ms"], 3), "batches_rewritten": cc["batches_rewritten"],
+                                  "batches_removed": cc["batches_removed"], "rows_purged": cc["rows_purged"],
+                                  "compaction_bytes_read": int(ct["bytes_read"]), "compaction_bytes_written": cc["bytes_written"],
+                                  "compaction_gbps": round((ct["bytes_read"] + cc["bytes_written"]) / (dev_ms * 1e6), 1) if dev_ms > 0 else None,
+                                  "store_bytes_before_compaction": bytes_before, "store_bytes_after_compaction": store.nbytes(),
+                                  "q1_kernel_ms_after_compaction": round(q1_compacted, 3),
+                                  "store_compressible_bytes": store.memory_info()[0], "store_slab_bytes": store.memory_info()[1]}), flush=True)
             store.close()
 
 
