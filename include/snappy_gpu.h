@@ -373,6 +373,25 @@ int sdx_store_memory_info(sd_store* s, int64_t* compressible_bytes, int64_t* sla
  * batch would be skipped.  Host only, no CUDA call (test hook: tests/test_stats_predicate.py compares it with the oracle). */
 int sdx_stats_pass(const sd_plan_desc* desc, const sd_literal* lits, int32_t nlits, const void* stats,
                    int64_t stats_len, int32_t stats_ncols, int32_t num_rows, int32_t* pass);
+/* what each kernel launch of a plan since its last sd_plan_reset ran: SDX_LAUNCH_WORDS int64 per launch, in launch order
+ * (test hook: the engine picks the decode path, kernel shape and group-table placement per batch and per launch; this
+ * reports the choice and changes nothing).  Word:
+ *   [0] accumulator (SDX_ACC_*)   [1] 1: the kernel variant with the per-row decode / overlay paths ran   [2] 1: the variant
+ *   with NULL literal flags ran   [3] stages of the shared-memory ring (0: direct loads)   [4] rows per tile
+ *   [5] rows per work item   [6] grid (CTAs)   [7] groups of the dense table (1 without one)   [8..11] batches of the launch
+ *   on the BATCH_ALL_FAST, BATCH_FAST_NULLS, BATCH_FAST_OVERLAY and general per-row paths   [12] SDX_REPLAY_*: why the launch
+ *   repeats an earlier one of the execution   [13] batches   [14] work items   [15] 0
+ * The first SDX_LAUNCH_LOG_MAX launches are kept.  *n = launches kept; min(cap, *n) records are written to out;
+ * SD_ERR_OVERFLOW when cap < *n. */
+#define SDX_LAUNCH_WORDS 16
+#define SDX_LAUNCH_LOG_MAX 4096
+enum { SDX_ACC_NOKEY = 0, SDX_ACC_PRIVATE = 1, SDX_ACC_SHARED_ATOMIC = 2, SDX_ACC_GLOBAL_ATOMIC = 3, SDX_ACC_HASH = 4,
+       SDX_ACC_REGTABLE = 5, SDX_ACC_ROWS = 6 /* projection / UPDATE / DELETE records */ };
+enum { SDX_REPLAY_NONE = 0,
+       SDX_REPLAY_HASH_SWITCH = 1,   /* the dense group table was given up for the hash table: earlier launches re-run  */
+       SDX_REPLAY_HASH_GROW = 2,     /* the hash table grew: every launch of the execution re-runs                      */
+       SDX_REPLAY_ROWS_GROW = 3 };   /* the projection / UPDATE / DELETE record buffer grew: every launch re-runs       */
+int sdx_plan_launch_log(sd_plan* p, int64_t* out, int32_t cap, int32_t* n);
 /* expand n raw LZ4 blocks with the engine's device kernel (bench/test hook used by tools/lz4_bench.py): uploads the
  * blocks, places output i at a 16-byte boundary + dst_misalign, runs `reps` launches timed with CUDA events
  * (ms_per_launch = their mean) and copies output i to outs[i] when outs != NULL.  `dense` selects the kernel variant:

@@ -22,6 +22,11 @@ SD_PLAN_MUTATE = 1   # sd_plan_desc.flags: UPDATE / DELETE plan
 METRIC_NAMES = ["numOutputRows", "numRowsBuffer", "columnBatchesSeen", "updatedColumnCount",
                 "deletedBatchCount", "columnBatchesSkipped", "aggTimeNs", "kernelLaunches",
                 "rowsScanned", "algorithmicBytes", "h2dBytes", "scanOutputRows"]
+# sdx_plan_launch_log records (include/snappy_gpu.h): SDX_ACC_*, the four batch paths, SDX_REPLAY_*
+SDX_LAUNCH_WORDS = 16
+LAUNCH_ACCUMULATORS = ["nokey", "private", "shared_atomic", "global_atomic", "hash", "regtable", "rows"]
+BATCH_PATHS = ["all_fast", "fast_nulls", "fast_overlay", "general"]
+LAUNCH_REPLAYS = [None, "hash_switch", "hash_grow", "rows_grow"]
 
 # sd_status
 SD_OK, SD_ERR_INVALID, SD_ERR_UNSUPPORTED, SD_ERR_CUDA, SD_ERR_OVERFLOW, SD_ERR_STATE = range(6)
@@ -270,6 +275,8 @@ def product_api() -> Api:
         L.sd_store_compact.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_double, C.POINTER(C.c_int64)]
         L.sdx_last_compaction_timing.restype = C.c_int
         L.sdx_last_compaction_timing.argtypes = [C.POINTER(C.c_double)]
+        L.sdx_plan_launch_log.restype = C.c_int
+        L.sdx_plan_launch_log.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.POINTER(C.c_int32)]
     return _product
 
 
@@ -532,6 +539,24 @@ class Plan:
 
     def kernel_name(self) -> str:
         return self.api.plan_kernel_name(self.h).decode()
+
+    def launch_log(self) -> List[Dict[str, object]]:
+        """What every kernel launch since the last reset ran (sdx_plan_launch_log), one dict per launch in launch order."""
+        f = self.api.lib.sdx_plan_launch_log
+        n = C.c_int32()
+        rc = f(self.h, None, 0, C.byref(n))
+        if rc not in (SD_OK, SD_ERR_OVERFLOW):
+            self.api.check(rc)
+        buf = (C.c_int64 * max(1, n.value * SDX_LAUNCH_WORDS))()
+        self.api.check(f(self.h, buf, n.value, C.byref(n)))
+        out = []
+        for i in range(n.value):
+            w = buf[i * SDX_LAUNCH_WORDS:(i + 1) * SDX_LAUNCH_WORDS]
+            out.append({"accumulator": LAUNCH_ACCUMULATORS[w[0]], "full_paths": bool(w[1]), "literal_nulls": bool(w[2]),
+                        "nstages": w[3], "tile_rows": w[4], "chunk_rows": w[5], "grid": w[6], "ngroups": w[7],
+                        "paths": dict(zip(BATCH_PATHS, w[8:12])), "replay": LAUNCH_REPLAYS[w[12]],
+                        "nbatches": w[13], "chunks": w[14]})
+        return out
 
     def set_option(self, option: int, value: int):
         self.api.check(self.api.plan_set_option(self.h, option, value))

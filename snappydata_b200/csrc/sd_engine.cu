@@ -268,6 +268,9 @@ struct StatEval {
 
 }  // namespace
 
+// batches of one launch per decode path: BATCH_ALL_FAST, BATCH_FAST_NULLS, BATCH_FAST_OVERLAY, general per-row decode
+struct PathCounts { int32_t n[4] = {0, 0, 0, 0}; };
+
 // =====================================================================================================
 struct sd_plan {
   int device = 0;
@@ -338,6 +341,7 @@ struct sd_plan {
   // descriptors -- as a new segment -- instead of re-deriving all of them (11 us per batch: 3.3 ms per query at 300 batches).
   struct ScanSegment {
     const void* d_batches = nullptr; const int32_t* d_prefix = nullptr; int nbatches = 0; int total_chunks = 0; int needs_slow = 0;
+    PathCounts paths;
     int64_t rows = 0, algo_bytes = 0, updated_cols = 0, deleted_batches = 0;
     size_t covered = 0;                          // batches of the store's snapshot this segment looked at (passing or skipped)
     std::vector<const StoredBatch*> batches;     // those that pass the stats check, in order
@@ -357,7 +361,7 @@ struct sd_plan {
   uint32_t hash_capacity = 0;
   uint64_t* d_hash_ident = nullptr;
   bool hash_init = false;
-  struct Launch { const void* d_batches; const int32_t* d_prefix; int nbatches; int total_chunks; int batch_base; int needs_slow; };
+  struct Launch { const void* d_batches; const int32_t* d_prefix; int nbatches; int total_chunks; int batch_base; int needs_slow; PathCounts paths; };
   // MODE_PROJECT output records + the batches of this execution (records carry a batch ordinal)
   uint8_t* d_out = nullptr;
   int64_t out_cap = 0;
@@ -370,6 +374,9 @@ struct sd_plan {
   std::vector<uint8_t> finished_rows;   // rows of the last sd_plan_finish (re-served when the caller's buffer was too small)
   int64_t finished_nrows = -1;
   std::vector<Launch> launch_log;
+  // what every kernel launch since the last reset ran (sdx_plan_launch_log): SDX_LAUNCH_WORDS words per launch
+  std::vector<int64_t> launch_records;
+  int replay_kind = SDX_REPLAY_NONE;   // why the launches being issued repeat earlier ones
   int64_t metrics[SD_NUM_METRICS] = {0};
   float agg_ms = 0;
   bool have_timing = false;
@@ -483,6 +490,7 @@ struct BuiltScan {
   const void* d_batches = nullptr; const int32_t* d_prefix = nullptr; int nbatches = 0; int total_chunks = 0;
   int64_t rows = 0, algo_bytes = 0, updated_cols = 0, deleted_batches = 0;
   int needs_slow = 0;   // some batch needs the kernel variant with the per-row paths
+  PathCounts paths;
   int needs_hash = 0;   // a key column of a dense-table plan is a raw (variable-width) string in some batch
 };
 
@@ -534,6 +542,7 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
     if (sb.dev_deletes) out->algo_bytes += 12 + 4 * (int64_t)sb.num_deletes;
     hdr->flags = all_fast ? BATCH_ALL_FAST : (base_fast ? BATCH_FAST_OVERLAY : ((simple_enc && !any_delta && !sb.dev_deletes) ? BATCH_FAST_NULLS : 0));
     if (!(hdr->flags == BATCH_ALL_FAST || (hdr->flags == BATCH_FAST_NULLS && p->kernel.staged))) out->needs_slow = 1;
+    out->paths.n[hdr->flags == BATCH_ALL_FAST ? 0 : hdr->flags == BATCH_FAST_NULLS ? 1 : hdr->flags == BATCH_FAST_OVERLAY ? 2 : 3]++;
     // per-batch tables: [int32 offset x nt][pad 8][uint64 kpack x nt][tables]; every table is indexed by the
     // unified dictionary code; key maps of <= 8 codes are also packed one byte per code into kpack
     if (nt) {
@@ -704,7 +713,7 @@ int plan_variant(sd_plan* p, int litnull, int slow, const KernelEntry** out) {
 }
 
 int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int nbatches, int total_chunks, int needs_slow,
-                const std::vector<const StoredBatch*>* blist = nullptr, int replay_batch_base = -1);
+                const PathCounts& paths, const std::vector<const StoredBatch*>* blist = nullptr, int replay_batch_base = -1);
 
 // A dense-table plan (dictionary-string keys) has to give up its table: too many key combinations, or a key column
 // arrives as raw variable-width strings (no dictionary ids).  The plan becomes its hash-table variant for good and
@@ -733,36 +742,45 @@ int switch_to_hash(sd_plan* p) {
   p->cache.valid = false;
   p->chunk_rows = CHUNK_ROWS;
   SD_CUDA(cudaMemsetAsync(p->d_counters, 0, 64, p->stream));
+  p->replay_kind = SDX_REPLAY_HASH_SWITCH;
   for (auto& l : earlier) {
     std::vector<const StoredBatch*> list(exec.begin() + l.batch_base, exec.begin() + l.batch_base + l.nbatches);
     BuiltScan bs;
     rc = build_scan(p, list, p->scratch, p->stream, &bs);
     if (rc) return rc;
-    rc = launch_scan(p, bs.d_batches, bs.d_prefix, bs.nbatches, bs.total_chunks, bs.needs_slow, &list);
+    rc = launch_scan(p, bs.d_batches, bs.d_prefix, bs.nbatches, bs.total_chunks, bs.needs_slow, bs.paths, &list);
     if (rc) return rc;
   }
+  p->replay_kind = SDX_REPLAY_NONE;
   return 0;
 }
 
+// a dense group table holds at most this many key combinations; beyond it the plan becomes its hash-table variant
+constexpr int64_t DENSE_GROUPS_MAX = 1 << 16;
+// key combinations of the dense table with the dictionaries seen so far
+int64_t dense_groups(const sd_plan* p) {
+  int64_t ng = 1;
+  for (size_t k = 0; k < p->spec.keys.size(); k++) ng *= std::max<int64_t>(1, (int64_t)p->key_vals[k].size());
+  return ng;
+}
+
 int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int nbatches, int total_chunks, int needs_slow,
-                const std::vector<const StoredBatch*>* blist, int replay_batch_base) {
+                const PathCounts& paths, const std::vector<const StoredBatch*>* blist, int replay_batch_base) {
   const bool replay = replay_batch_base >= 0;
   if (!replay && p->spec.mode == MODE_GROUPS) {   // dense table still possible with the dictionaries seen so far?
-    int64_t ng = 1;
-    for (size_t k = 0; k < p->spec.keys.size(); k++) ng *= std::max<int64_t>(1, (int64_t)p->key_vals[k].size());
-    if (ng > (1 << 16)) {
+    if (dense_groups(p) > DENSE_GROUPS_MAX) {
       if (!blist) return set_error(SD_ERR_STATE, "dense group table overflow without a batch list");
       int rc = switch_to_hash(p);
       if (rc) return rc;
       BuiltScan bs;
       rc = build_scan(p, *blist, p->scratch, p->stream, &bs);
       if (rc) return rc;
-      return launch_scan(p, bs.d_batches, bs.d_prefix, bs.nbatches, bs.total_chunks, bs.needs_slow, blist);
+      return launch_scan(p, bs.d_batches, bs.d_prefix, bs.nbatches, bs.total_chunks, bs.needs_slow, bs.paths, blist);
     }
   }
   int batch_base = replay ? replay_batch_base : (int)p->exec_batches.size();
   if (!replay && p->spec.mode != MODE_NOKEY) {
-    p->launch_log.push_back({d_batches, d_prefix, nbatches, total_chunks, batch_base, needs_slow});
+    p->launch_log.push_back({d_batches, d_prefix, nbatches, total_chunks, batch_base, needs_slow, paths});
     if (blist) p->exec_batches.insert(p->exec_batches.end(), blist->begin(), blist->end());
   }
   p->finished_nrows = -1;
@@ -932,6 +950,16 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   if (own_pair) SD_CUDA(cudaEventRecord(p->ev_pairs[p->ev_used].first, p->stream));
   if (!p->have_timing) SD_CUDA(cudaEventRecord(p->ev_start, p->stream));
   { int rc = kernel_launch(*k, grid, smem, p->stream, kargs); if (rc) return rc; }
+  if (p->launch_records.size() < (size_t)SDX_LAUNCH_LOG_MAX * SDX_LAUNCH_WORDS) {
+    const int acc = sp.mode == MODE_NOKEY ? SDX_ACC_NOKEY : sp.mode == MODE_HASH ? SDX_ACC_HASH
+                  : (sp.mode == MODE_PROJECT || sp.mode == MODE_MUTATE) ? SDX_ACC_ROWS
+                  : table_mode == TABLE_PRIVATE ? SDX_ACC_PRIVATE : table_mode == TABLE_SHARED_ATOMIC ? SDX_ACC_SHARED_ATOMIC
+                  : table_mode == TABLE_GLOBAL_ATOMIC ? SDX_ACC_GLOBAL_ATOMIC : SDX_ACC_REGTABLE;
+    const int64_t rec[SDX_LAUNCH_WORDS] = {acc, k == &p->variant[2] || k == &p->variant[3], k == &p->variant[1] || k == &p->variant[3],
+                                           nstages, k->tile_rows, p->chunk_rows, grid, ngroups, paths.n[0], paths.n[1], paths.n[2],
+                                           paths.n[3], p->replay_kind, nbatches, total_chunks, 0};
+    p->launch_records.insert(p->launch_records.end(), rec, rec + SDX_LAUNCH_WORDS);
+  }
   SD_CUDA(cudaEventRecord(p->ev_stop, p->stream));
   if (own_pair) { SD_CUDA(cudaEventRecord(p->ev_pairs[p->ev_used].second, p->stream)); p->ev_used++; }
   p->have_timing = true;
@@ -973,7 +1001,7 @@ int flush_pending(sd_plan* p) {
   p->metrics[3] += bs.updated_cols;
   p->metrics[4] += bs.deleted_batches;
   p->metrics[9] += bs.algo_bytes;
-  rc = launch_scan(p, bs.d_batches, bs.d_prefix, bs.nbatches, bs.total_chunks, bs.needs_slow, &list);
+  rc = launch_scan(p, bs.d_batches, bs.d_prefix, bs.nbatches, bs.total_chunks, bs.needs_slow, bs.paths, &list);
   p->pending.clear();
   p->pending_bytes = 0;
   return rc;
@@ -1013,12 +1041,13 @@ int resolve_kernel(const sd_plan_desc& desc, const CodegenOptions& opt, int devi
   if (rc) return set_error(rc, "%s", err.c_str());
   static std::mutex registry_mutex;   // plans are created concurrently from many task threads
   std::lock_guard<std::mutex> lock(registry_mutex);
-  for (auto& k : kernel_registry()) if (k.signature == spec.signature) { *out = k; if (spec_out) *spec_out = spec; return 0; }
+  for (auto& k : kernel_registry()) if (k.signature == spec.signature) { *out = k; out->tile_rows = THREADS * spec.rpt; if (spec_out) *spec_out = spec; return 0; }
   KernelEntry k;
   rc = jit_compile(spec, device, k);
   if (rc) return rc;
   kernel_registry().push_back(k);
   *out = k;
+  out->tile_rows = THREADS * spec.rpt;
   if (spec_out) *spec_out = spec;
   return 0;
 }
@@ -1100,7 +1129,9 @@ int finish_hash(sd_plan* p) {
     int rc = hash_ensure(p, ncap);
     if (rc) return rc;
     SD_CUDA(cudaMemsetAsync(p->d_counters, 0, 64, p->stream));
-    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, nullptr, l.batch_base); if (rc) return rc; }
+    p->replay_kind = SDX_REPLAY_HASH_GROW;
+    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, l.paths, nullptr, l.batch_base); if (rc) return rc; }
+    p->replay_kind = SDX_REPLAY_NONE;
   }
   const uint32_t count = flags[8];
   // compact -> host
@@ -1289,7 +1320,9 @@ int finish_project(sd_plan* p) {
     if (rc) return rc;
     SD_CUDA(cudaMemsetAsync(p->d_out_count, 0, 8, p->stream));
     SD_CUDA(cudaMemsetAsync(p->d_counters, 0, 64, p->stream));
-    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, nullptr, l.batch_base); if (rc) return rc; }
+    p->replay_kind = SDX_REPLAY_ROWS_GROW;
+    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, l.paths, nullptr, l.batch_base); if (rc) return rc; }
+    p->replay_kind = SDX_REPLAY_NONE;
   }
   {
     bool done = false;
@@ -1598,7 +1631,9 @@ int sd::mutation_scan(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
     if (rc) return rc;
     SD_CUDA(cudaMemsetAsync(p->d_out_count, 0, 8, p->stream));
     SD_CUDA(cudaMemsetAsync(p->d_counters, 0, 64, p->stream));
-    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, nullptr, l.batch_base); if (rc) return rc; }
+    p->replay_kind = SDX_REPLAY_ROWS_GROW;
+    for (auto& l : p->launch_log) { rc = launch_scan(p, l.d_batches, l.d_prefix, l.nbatches, l.total_chunks, l.needs_slow, l.paths, nullptr, l.batch_base); if (rc) return rc; }
+    p->replay_kind = SDX_REPLAY_NONE;
   }
   update_agg_time(p);
   p->metrics[6] = (int64_t)(p->agg_ms * 1e6);
@@ -1659,9 +1694,12 @@ static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
     BuiltScan bs;
     int rc2 = build_scan(p, list, p->cache_arena, p->stream, &bs);
     if (rc2) return rc2;
-    if (bs.needs_hash && p->spec.mode == MODE_GROUPS) return -1000;   // the caller switches the plan and rebuilds everything
+    // a key column without dictionary ids, or more key combinations than a dense table holds: the caller switches the plan
+    // to the hash table and rebuilds every segment (descriptors built for the dense kernel carry key-id tables where the
+    // hash kernel reads string-record addresses, so no segment built before the switch may be launched after it)
+    if (p->spec.mode == MODE_GROUPS && (bs.needs_hash || dense_groups(p) > DENSE_GROUPS_MAX)) return -1000;
     seg->d_batches = bs.d_batches; seg->d_prefix = bs.d_prefix; seg->nbatches = bs.nbatches; seg->total_chunks = bs.total_chunks;
-    seg->needs_slow = bs.needs_slow; seg->rows = bs.rows; seg->algo_bytes = bs.algo_bytes;
+    seg->needs_slow = bs.needs_slow; seg->paths = bs.paths; seg->rows = bs.rows; seg->algo_bytes = bs.algo_bytes;
     seg->updated_cols = bs.updated_cols; seg->deleted_batches = bs.deleted_batches;
     seg->covered = snapshot.size() - from;
     seg->batches.swap(list);
@@ -1706,7 +1744,14 @@ static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
       }
     }
   }
-  if (!rebuilt && !(same_query && c.version == snap_version)) {
+  // (the store's address and version do not identify its batches: a store created where a destroyed one lived starts at the
+  // same version; batch uids are never reused)
+  auto same_batches = [&]() {
+    if (snapshot.size() != c.snap_uids.size()) return false;
+    for (size_t i = 0; i < snapshot.size(); i++) if (snapshot[i]->uid != c.snap_uids[i]) return false;
+    return true;
+  };
+  if (!rebuilt && !(same_query && c.version == snap_version && same_batches())) {
     // (re)build everything: stats skipping + descriptors + tables, kept on the device for repeated executions
     c.valid = false;
     c.segs.clear();
@@ -1741,7 +1786,7 @@ static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
   bool launched = false;
   for (const sd_plan::ScanSegment& seg : c.segs) {
     if (seg.nbatches == 0 && launched) continue;
-    rc = launch_scan(p, seg.d_batches, seg.d_prefix, seg.nbatches, seg.total_chunks, seg.needs_slow, &seg.batches);
+    rc = launch_scan(p, seg.d_batches, seg.d_prefix, seg.nbatches, seg.total_chunks, seg.needs_slow, seg.paths, &seg.batches);
     if (rc) return rc;
     launched = true;
   }
@@ -1852,6 +1897,8 @@ int sd_plan_reset(sd_plan* p) {
   p->result_init = false;
   p->hash_init = false;
   p->launch_log.clear();
+  p->launch_records.clear();
+  p->replay_kind = SDX_REPLAY_NONE;
   p->exec_batches.clear();
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
@@ -1883,6 +1930,15 @@ int sd_plan_reset(sd_plan* p) {
 int sd_plan_metrics(sd_plan* p, int64_t out[SD_NUM_METRICS]) {
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
   memcpy(out, p->metrics, sizeof(p->metrics));
+  return 0;
+}
+
+int sdx_plan_launch_log(sd_plan* p, int64_t* out, int32_t cap, int32_t* n) {
+  if (!p || !n || cap < 0 || (cap > 0 && !out)) return set_error(SD_ERR_INVALID, "sdx_plan_launch_log: bad arguments");
+  const int32_t have = (int32_t)(p->launch_records.size() / SDX_LAUNCH_WORDS);
+  *n = have;
+  if (cap > 0) memcpy(out, p->launch_records.data(), (size_t)std::min(cap, have) * SDX_LAUNCH_WORDS * 8);
+  if (cap < have) return set_error(SD_ERR_OVERFLOW, "sdx_plan_launch_log: %d records", have);
   return 0;
 }
 

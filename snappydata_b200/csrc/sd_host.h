@@ -36,6 +36,7 @@ struct KernelEntry {
   size_t tile_smem;      // sizeof(TileSmem<PLAN>) rounded up to 16
   int staged = 0;        // PLAN::STAGES > 0: producer warp + shared-memory ring (block = THREADS + 32)
   size_t stage_bytes = 0;
+  int tile_rows = 0;     // THREADS * PLAN::RPT (set by the engine when it resolves the kernel)
   std::string origin;    // "aot" | "jit"
   std::string name;      // Plan_<fnv1a(signature)>: the generated struct's name
 };
