@@ -284,11 +284,31 @@ int sd_plan_delete_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int
  *      and has no deltas and no mask: its row ordinals are the live rows renumbered from 0, and later UPDATE / DELETE
  *      statements address those.  Serialised with UPDATE / DELETE; works on the batches present when it starts; everything
  *      is installed in one step under the store's lock (a scan sees all of it or none).  Superseded bytes stay in the arena
- *      until the store is destroyed.  Refused with nothing installed: a column that must be rewritten but that the engine
+ *      until sd_store_reclaim frees them or the store is destroyed.  Refused with nothing installed: a column that must be rewritten but that the engine
  *      cannot decode -- an Uncompressed (variable-width) STRING column, a column the scan does not support --
  *      (SD_ERR_UNSUPPORTED, naming batch and column); a negative or NaN min_dirty_fraction, a null store (SD_ERR_INVALID).
  *      out[0] batches rewritten, out[1] batches removed, out[2] deleted rows purged, out[3] bytes written to the store's arena */
 int sd_store_compact(sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, double min_dirty_fraction, int64_t out[4]);
+
+/* ---- reclaim: give back the device memory of superseded batch versions --------------------------------------------------
+ *      UPDATE / DELETE / compaction leave every version they replace in the store's arena, because a scan of an older
+ *      snapshot may still read it.  This call frees what no open scan can read.  Live bytes are the allocations of every
+ *      current batch version plus those of replaced versions that an open scan may still read; a scan is open from its
+ *      snapshot (sd_plan_scan_store) until its result is materialised (sd_plan_finish), sd_plan_reset or sd_plan_destroy.
+ *      Every slab the store holds when the call starts is considered (the slab being allocated from is closed first, so
+ *      max_live_fraction = 1 can empty every slab): a slab without live bytes is freed without copying; a slab whose live
+ *      bytes are at most max_live_fraction x its size is evacuated -- the live bytes of current versions are copied on the
+ *      device into fresh slabs of the same arena, emptiest slabs first, in rounds of at most one destination slab, and each
+ *      round installs new versions of the batches it moved (same bytes, rows, bucket, batch id, stats, deltas and mask at
+ *      new addresses, new identity) in one step under the store's lock.  A source slab an open scan can still read is
+ *      deferred: a later call frees it.  0 only frees dead slabs; 1 repacks everything.  sd_store_bytes drops by the bytes
+ *      that were allocated in the freed slabs.  Serialised with UPDATE / DELETE / compaction and the device encoder;
+ *      sd_store_put_batch may run meanwhile.  A failing round installs and frees nothing (rounds already installed stay,
+ *      their bytes identical; the error says so); a device pointer of a batch that lies in none of its recorded allocations
+ *      fails the call before anything is copied (SD_ERR_STATE, naming batch and column); a null store or a NaN, negative or
+ *      > 1 fraction is refused with nothing changed (SD_ERR_INVALID).
+ *      out[0] slabs freed, out[1] slab bytes freed, out[2] bytes copied, out[3] slabs deferred */
+int sd_store_reclaim(sd_store* s, double max_live_fraction, int64_t out[4]);
 
 /* ---- final merge (SnappyHashAggregateExec(Final) / CollectAggregateExec.executeCollect,
  *      core/execution/aggregate/CollectAggregateExec.scala:67-121): merges partial rows of all
@@ -361,6 +381,12 @@ int sdx_last_mutation_timing(double out[6]);
 /* the calling thread's last sd_store_compact: [0] materialise ms [1] encode ms (device events) [2] host layout + install ms
  * [3] whole call ms (host clock) [4] rows of the rewritten batches [5] bytes read (columns, deltas, delete masks) */
 int sdx_last_compaction_timing(double out[6]);
+/* the calling thread's last sd_store_reclaim: [0] inventory + planning ms (host) [1] copy ms (device events) [2] install ms
+ * (host) [3] free ms (host) [4] whole call ms (host clock) [5] rounds */
+int sdx_last_reclaim_timing(double out[6]);
+/* bytes in the device allocations of the store's current batch versions (out[0]) and of the replaced versions kept for open
+ * scans that the current ones do not share (out[1]) */
+int sdx_store_extent_bytes(sd_store* s, int64_t out[2]);
 /* stats row (UnsafeRow) of a resident batch */
 int sdx_store_get_stats(sd_store* s, int64_t batch_index, void* out, int64_t cap, int64_t* out_len);
 int sdx_store_batch_info(sd_store* s, int64_t batch_index, int32_t* num_rows, int32_t* bucket_id,

@@ -297,6 +297,20 @@ JNIEXPORT void JNICALL JFN(compactStore)(JNIEnv* env, jobject self, jlong store,
   (*env)->SetLongArrayRegion(env, out, 0, 4, o);
 }
 
+/* reclaim: frees the device memory of superseded batch versions, after a compaction typically (sd_store_reclaim); out
+ * (length >= 4): slabs freed, slab bytes freed, bytes copied, slabs deferred (an unfinished scan still reads them) */
+JNIEXPORT void JNICALL JFN(reclaimStore)(JNIEnv* env, jobject self, jlong store, jdouble maxLiveFraction, jlongArray out) {
+  (void)self;
+  if (out == NULL || (*env)->GetArrayLength(env, out) < 4) {
+    throw_msg(env, "java/lang/IllegalArgumentException", "reclaimStore: out must hold 4 longs");
+    return;
+  }
+  int64_t counts[4] = {0, 0, 0, 0};
+  if (sd_store_reclaim((sd_store*)(intptr_t)store, (double)maxLiveFraction, counts)) { throw_last(env); return; }
+  jlong o[4] = {(jlong)counts[0], (jlong)counts[1], (jlong)counts[2], (jlong)counts[3]};
+  (*env)->SetLongArrayRegion(env, out, 0, 4, o);
+}
+
 /* ---- the cross-partition exchange (INTEGRATION.md section 4b) ------------------------------------------------------ */
 /* rank 0 fills a 128-byte id; the caller broadcasts it (a Spark broadcast variable) */
 JNIEXPORT void JNICALL JFN(commUniqueId)(JNIEnv* env, jobject self, jbyteArray out128) {

@@ -60,6 +60,11 @@ object SnappyGpuNative {
     * out(0) batches rewritten, out(1) removed, out(2) deleted rows purged, out(3) bytes written.  Rewritten batches number
     * their live rows from 0: later UPDATE / DELETE positions and any JVM-side mirror of the bytes follow the new version */
   @native def compactStore(store: Long, bucketIds: Array[Int], minDirtyFraction: Double, out: Array[Long]): Unit
+  /** gives back the device memory of superseded batch versions; call it after a compaction.  Slabs at most
+    * maxLiveFraction live are emptied into fresh ones first (0: only dead slabs are freed, 1: everything is repacked).
+    * A scan pins what it may read until its plan finishes, is reset or destroyed: such slabs are deferred to a later call.
+    * out(0) slabs freed, out(1) slab bytes freed, out(2) bytes copied, out(3) slabs deferred */
+  @native def reclaimStore(store: Long, maxLiveFraction: Double, out: Array[Long]): Unit
 
   // ---- the exchange between co-located GPU partitions (INTEGRATION.md 4b) ------------------------------------------------
   /** rank 0 calls this and broadcasts the 128 bytes; every rank passes them to commCreate */

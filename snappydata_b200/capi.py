@@ -275,6 +275,12 @@ def product_api() -> Api:
         L.sd_store_compact.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_double, C.POINTER(C.c_int64)]
         L.sdx_last_compaction_timing.restype = C.c_int
         L.sdx_last_compaction_timing.argtypes = [C.POINTER(C.c_double)]
+        L.sd_store_reclaim.restype = C.c_int
+        L.sd_store_reclaim.argtypes = [C.c_void_p, C.c_double, C.POINTER(C.c_int64)]
+        L.sdx_last_reclaim_timing.restype = C.c_int
+        L.sdx_last_reclaim_timing.argtypes = [C.POINTER(C.c_double)]
+        L.sdx_store_extent_bytes.restype = C.c_int
+        L.sdx_store_extent_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
         L.sdx_plan_launch_log.restype = C.c_int
         L.sdx_plan_launch_log.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.POINTER(C.c_int32)]
     return _product
@@ -742,6 +748,20 @@ class Store:
         self.api.check(self.api.lib.sd_store_compact(self.h, b if nb else None, nb, float(min_dirty_fraction), out))
         return dict(zip(("batches_rewritten", "batches_removed", "rows_purged", "bytes_written"), (int(x) for x in out)))
 
+    def reclaim(self, max_live_fraction: float = 0.0) -> Dict[str, int]:
+        """Give back the device memory of superseded batch versions (sd_store_reclaim): slabs nothing live lies in are
+        freed, slabs at most `max_live_fraction` live are emptied into fresh ones first.  Slabs an unfinished scan can
+        still read are deferred to a later call."""
+        out = (C.c_int64 * 4)()
+        self.api.check(self.api.lib.sd_store_reclaim(self.h, float(max_live_fraction), out))
+        return dict(zip(("slabs_freed", "bytes_freed", "bytes_moved", "slabs_deferred"), (int(x) for x in out)))
+
+    def extent_bytes(self):
+        """(bytes of the current batch versions' allocations, bytes only replaced versions kept for open scans hold)."""
+        out = (C.c_int64 * 2)()
+        self.api.check(self.api.lib.sdx_store_extent_bytes(self.h, out))
+        return int(out[0]), int(out[1])
+
     def get_deletes(self, batch_index: int) -> bytes:
         """A batch's delete mask [0][numBaseRows][numDeletes][positions] (sdx_store_get_deletes)."""
         ln = C.c_int64()
@@ -765,3 +785,10 @@ def last_compaction_timing(api: Api) -> Dict[str, float]:
     out = (C.c_double * 6)()
     api.check(api.lib.sdx_last_compaction_timing(out))
     return dict(zip(("materialise_ms", "encode_ms", "host_ms", "compaction_ms", "rows_read", "bytes_read"), list(out)))
+
+
+def last_reclaim_timing(api: Api) -> Dict[str, float]:
+    """Host and device times of the calling thread's last reclaim (sdx_last_reclaim_timing)."""
+    out = (C.c_double * 6)()
+    api.check(api.lib.sdx_last_reclaim_timing(out))
+    return dict(zip(("plan_ms", "copy_ms", "install_ms", "free_ms", "reclaim_ms", "rounds"), list(out)))

@@ -278,6 +278,7 @@ int compact_round(sd_store* s, cudaStream_t st, cudaEvent_t* ev, std::vector<Bat
       nb->num_rows = round[r]->n_live;
       nb->dev_deletes = nullptr; nb->num_deletes = 0; nb->has_deltas = false; nb->gone = false;
       stats[r].resize(round[r]->cols.size());
+      ExtentRecorder rec(s->arena, &nb->extents);   // (the rewritten columns' old extents are pruned at install)
       for (size_t q = 0; q < round[r]->cols.size(); q++) {
         ColWork& cw = round[r]->cols[q];
         if ((rc = enc_layout(s, st, pin, cw.job, nb->cols[cw.table_col], stats[r][q]))) return rc;

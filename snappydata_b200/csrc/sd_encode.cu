@@ -513,10 +513,13 @@ extern "C" int sd_store_encode_batch(sd_store* s, int32_t num_rows, const sd_raw
   std::vector<ColStat> stats(s->schema.size());
   std::vector<ColStat*> job_stats;
   std::unique_lock<std::mutex> store_lock(s->mu);   // phase 2: arena placement + the small side uploads of upload_column
-  for (Work& w : work) {
-    int rc = enc_layout(s, st, s->enc_host, w.job, sb->cols[w.job.table_col], stats[w.job.table_col]);
-    if (rc) return rc;
-    job_stats.push_back(&stats[w.job.table_col]);
+  {
+    ExtentRecorder rec(s->arena, &sb->extents);
+    for (Work& w : work) {
+      int rc = enc_layout(s, st, s->enc_host, w.job, sb->cols[w.job.table_col], stats[w.job.table_col]);
+      if (rc) return rc;
+      job_stats.push_back(&stats[w.job.table_col]);
+    }
   }
   // the side uploads (null words, prefixes of "nulls before") went over the store's copy stream: order the encoder after them
   SD_CUDA(cudaEventRecord(s->enc_event, s->copy_stream));

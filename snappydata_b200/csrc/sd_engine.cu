@@ -371,6 +371,9 @@ struct sd_plan {
   int64_t dev_rows_len = -1;      // >= 0: the finished rows of this execution are roww.d_rows[0, dev_rows_len) (not finished_rows)
   unsigned long long* d_out_count = nullptr;
   std::vector<const StoredBatch*> exec_batches;
+  // the stores this execution may still read (hash-table string keys, MIN / MAX(STRING) slots and projected strings refer to
+  // records in a store's memory): released once the result is materialised, by sd_plan_reset and sd_plan_destroy
+  HeldPins pins;
   std::vector<uint8_t> finished_rows;   // rows of the last sd_plan_finish (re-served when the caller's buffer was too small)
   int64_t finished_nrows = -1;
   std::vector<Launch> launch_log;
@@ -1645,6 +1648,8 @@ int sd::mutation_scan(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
   out->scan_ms = p->agg_ms;
   p->finished_nrows = (int64_t)count;
   p->metrics[0] = (int64_t)count;
+  // the statement goes on reading these batches, but under the store's mutate_mu, which keeps sd_store_reclaim out
+  p->pins.release();
   return 0;
 }
 
@@ -1669,6 +1674,7 @@ static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
     snapshot.reserve(s->batches.size());
     for (auto& sbp : s->batches) snapshot.push_back(sbp.get());
     snap_version = s->version;
+    p->pins.take(s->pins, snap_version);   // sd_store_reclaim frees nothing this snapshot can read until the pin is released
   }
   for (auto& c : p->spec.cols) {
     if (c.table_ordinal < 0 || c.table_ordinal >= (int)s->schema.size()) return set_error(SD_ERR_INVALID, "plan column ordinal %d outside the store schema", c.table_ordinal);
@@ -1865,6 +1871,9 @@ static int collect_partial_rows(sd_plan* p) {
   rc = mode == MODE_HASH ? finish_hash(p) : mode == MODE_PROJECT ? finish_project(p) : finish_dense(p);
   if (rc) return rc;
   p->metrics[0] = p->finished_nrows;
+  // the rows are host bytes, or device rows holding their own string bytes, and the stream has drained: the scan reads no
+  // store memory any more (a cached plan sitting idle between queries pins nothing)
+  p->pins.release();
   return 0;
 }
 
@@ -1892,6 +1901,7 @@ int sd_plan_reset(sd_plan* p) {
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
   SD_CUDA(cudaSetDevice(p->device));
   SD_CUDA(cudaStreamSynchronize(p->stream));
+  p->pins.release();
   p->pending.clear();
   p->pending_bytes = 0;
   p->result_init = false;
@@ -1946,6 +1956,7 @@ void sd_plan_destroy(sd_plan* p) {
   if (!p) return;
   cudaSetDevice(p->device);
   if (p->stream) cudaStreamSynchronize(p->stream);
+  p->pins.release();   // (the registry outlives a store destroyed before this plan)
   if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
   if (p->ev_start) cudaEventDestroy(p->ev_start);
   if (p->ev_stop) cudaEventDestroy(p->ev_stop);

@@ -172,6 +172,7 @@ extern "C" int sdx_store_gen_lineitem(sd_store* s, int64_t first_row, int64_t nr
     sb->batch_id = (int64_t)(firsts[b] / rows_per_batch);
     sb->bucket_id = (int32_t)(sb->batch_id % nbuckets);
     sb->cols.resize(s->schema.size());
+    ExtentRecorder rec(s->arena, &sb->extents);
     for (int k = 0; k < 7; k++) {
       if (!((column_mask >> kOrdinal[k]) & 1)) continue;
       StoredCol& c = sb->cols[kOrdinal[k]];

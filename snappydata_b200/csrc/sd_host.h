@@ -5,11 +5,14 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <climits>
 #include <cstdint>
 #include <functional>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -98,6 +101,8 @@ void comm_destroy(void* c);
 int comm_all_gather_bytes(void* c, const void* d_send, void* d_recv, size_t bytes_per_rank, cudaStream_t stream);
 
 // ---- device memory arena: bump allocation out of large slabs ---------------------------------------
+// one allocation of a store's arena that a batch version owns (sd_reclaim.cu moves and frees by these)
+struct Extent { uint8_t* ptr; size_t bytes; };
 struct Arena {
   int device = 0;
   size_t slab_bytes = size_t(512) << 20;
@@ -111,16 +116,29 @@ struct Arena {
     bool vmm;                   // cuMemCreate + cuMemMap (else cudaMalloc)
     bool compressed;            // the driver granted generic compression
     unsigned long long handle;  // CUmemGenericAllocationHandle of a vmm slab
+    size_t used;                // bytes allocated out of it
   };
   std::vector<Slab> slabs;
   size_t cur_slab = 0;
   size_t cur_off = 0;
   size_t used = 0;
+  // non-null: every allocation is appended here as an extent (ExtentRecorder scopes it to one batch version)
+  std::vector<Extent>* record = nullptr;
   // returns p with (p + misalign) % align == 0, or nullptr (error set)
   uint8_t* alloc(size_t n, size_t align = 256, size_t misalign = 0);
   void reset();     // keep slabs, forget allocations
   void release();   // free slabs
+  // stop allocating from the current slab: the next allocation opens a fresh one
+  void close_slab() { cur_slab = slabs.size(); cur_off = 0; }
+  // take slab i out of the arena (its allocated bytes leave `used`); the caller frees it with free_slab
+  Slab detach_slab(size_t i);
+  static void free_slab(int device, const Slab& s);
   ~Arena() { release(); }
+};
+struct ExtentRecorder {
+  Arena& a;
+  ExtentRecorder(Arena& arena, std::vector<Extent>* to) : a(arena) { a.record = to; }
+  ~ExtentRecorder() { a.record = nullptr; }
 };
 
 // page-locked host staging for small uploads (descriptors, tables) that must not block the submitting thread:
@@ -176,6 +194,79 @@ struct StoredBatch {
   bool has_deltas = false;
   bool positional = false;                // cols are indexed by the plan's scan column (private store)
   bool gone = false;                      // every row deleted (ColumnDelta.checkBatchDeleted): no scan reads it
+  // the arena allocations this version's device pointers lie in (a new version inherits those of the columns it keeps;
+  // store_install drops the ones no pointer refers to any more)
+  std::vector<Extent> extents;
+  int64_t retired_at = -1;                // store version that replaced or removed it (scans of an older snapshot may read it)
+};
+
+// Every device pointer a batch version owns, in one place: the reclaim's inventory and its rebase both walk this list
+// (sd_reclaim.cu).  f(uintptr_t address, int table_col, const char* field) returns the address the field is to hold; the
+// batch's delete mask reports column -1.  The device-resident DevDelta structs (dev_delta[]) hold copies of the host
+// StoredDelta::dev pointers; whoever moves them rewrites them from the host copies.
+template <class F>
+void visit_device_pointers(StoredBatch& b, F&& f) {
+  auto one = [&](auto& field, int col, const char* what) {
+    if (!field) return;
+    typedef typename std::remove_reference<decltype(field)>::type P;
+    field = (P)f((uintptr_t)field, col, what);
+  };
+  for (int c = 0; c < (int)b.cols.size(); c++) {
+    StoredCol& sc = b.cols[c];
+    if (!sc.present) continue;
+    one(sc.dev_base, c, "dev_base");
+    one(sc.dev.data, c, "data");
+    one(sc.dev.nulls, c, "nulls");
+    one(sc.dev.tile_nulls, c, "tile_nulls");
+    one(sc.dev.dict, c, "dict");
+    one(sc.dev.run_ends, c, "run_ends");
+    one(sc.dev.delta0, c, "delta0");
+    one(sc.dev.delta1, c, "delta1");
+    for (int d = 0; d < 2; d++) {
+      StoredDelta& sd = sc.delta[d];
+      if (sd.present) {
+        one(sd.dev.positions, c, "delta positions");
+        one(sd.dev.data, c, "delta data");
+        one(sd.dev.nulls, c, "delta nulls");
+        one(sd.dev.dict, c, "delta dict");
+      }
+      one(sc.dev_delta[d], c, "dev_delta");
+    }
+    for (int64_t& r : sc.dict_rec_ptr) one(r, c, "dict_rec_ptr");
+  }
+  one(b.dev_deletes, -1, "dev_deletes");
+}
+// drop the extents no device pointer of the version lies in (those a replaced delta / mask / column left behind)
+void prune_extents(StoredBatch& b);
+
+// Scans that may still read a store's memory: the store version each one saw when it took its snapshot.  Shared between
+// the store and the plans that scanned it (either may be destroyed first).
+struct ScanPins {
+  std::mutex mu;
+  std::multiset<int64_t> versions;
+  int64_t oldest() {
+    std::lock_guard<std::mutex> lock(mu);
+    return versions.empty() ? INT64_MAX : *versions.begin();
+  }
+};
+// the pins a plan holds: at most one per store, the oldest (taken at its first snapshot of the execution)
+struct HeldPins {
+  std::vector<std::pair<std::shared_ptr<ScanPins>, int64_t>> held;
+  void take(const std::shared_ptr<ScanPins>& r, int64_t version) {
+    for (auto& h : held) if (h.first == r) return;
+    std::lock_guard<std::mutex> lock(r->mu);
+    r->versions.insert(version);
+    held.emplace_back(r, version);
+  }
+  void release() {
+    for (auto& h : held) {
+      std::lock_guard<std::mutex> lock(h.first->mu);
+      auto it = h.first->versions.find(h.second);
+      if (it != h.first->versions.end()) h.first->versions.erase(it);
+    }
+    held.clear();
+  }
+  ~HeldPins() { release(); }
 };
 
 }  // namespace sd
@@ -195,11 +286,14 @@ struct sd_store {
   int next_stream = 0;
   cudaEvent_t extra_done[4] = {nullptr, nullptr, nullptr, nullptr};
   std::vector<std::unique_ptr<sd::StoredBatch>> batches;
-  // UPDATE / DELETE / compaction replace a batch by a new version at the same index (compaction also drops fully deleted
-  // batches); the old one stays alive here until the store is destroyed (scans hold raw pointers into their snapshot).
-  // `mutate_mu` serialises the statements and compactions on this store.
+  // UPDATE / DELETE / compaction / reclaim replace a batch by a new version at the same index (compaction also drops fully
+  // deleted batches); the old one stays alive here (scans hold raw pointers into their snapshot) until sd_store_reclaim finds
+  // that no open scan can read it, or the store is destroyed.  `mutate_mu` serialises the statements, compactions and
+  // reclaims on this store.
   std::vector<std::unique_ptr<sd::StoredBatch>> retired;
   std::mutex mutate_mu;
+  // the open scans of this store (taken with the snapshot under `mu`, released when the scan's result is materialised)
+  std::shared_ptr<sd::ScanPins> pins = std::make_shared<sd::ScanPins>();
   int64_t version = 0;
   int64_t h2d_bytes = 0;
   bool retain_buffers = false;   // SD_OPT_RETAIN_BUFFERS: no per-put synchronisation of the copy stream
@@ -268,8 +362,9 @@ struct DevScratch {
 
 // install new batch versions and drop batches, all under ONE hold of the store's lock (a scan's snapshot sees every change
 // or none): fresh[i].second replaces fresh[i].first at its index, `remove` leaves the store; the replaced and removed
-// versions move to `retired` (scans of an older snapshot may still read them).  SD_ERR_STATE, nothing changed, when one
-// of the named batches is no longer in the store (sd_store.cu)
+// versions move to `retired` (scans of an older snapshot may still read them) marked with the new store version; the
+// fresh versions' extents are pruned.  SD_ERR_STATE, nothing changed, when one of the named batches is no longer in the
+// store (sd_store.cu)
 typedef std::vector<std::pair<const StoredBatch*, std::unique_ptr<StoredBatch>>> FreshBatches;
 int store_install(sd_store* s, FreshBatches& fresh, const std::vector<const StoredBatch*>& remove, const char* what);
 

@@ -437,12 +437,14 @@ int run_statement(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nb
   if (upd && ((rc = ds.get(&d_tval, 8 * tmp_entries)) || (rc = ds.get(&d_tnull, tmp_entries)))) return rc;
   std::vector<DevDelta> devd(pairs.size());
   DevDelta* d_devd = nullptr;
+  std::vector<std::vector<Extent>> new_extents(nb);   // per batch: the allocations its new version adds
   {
     std::lock_guard<std::mutex> lock(s->mu);
     size_t toff = 0;
     for (size_t i = 0; i < pairs.size(); i++) {
       const PairCounts& c = counts[i];
       if (!c.n_new) continue;
+      ExtentRecorder rec(s->arena, &new_extents[i / T]);
       MergePair& mp = pairs[i];
       mp.out_pos = reinterpret_cast<int32_t*>(s->arena.alloc(4 * (size_t)c.n_union + 16, 16));
       if (!mp.out_pos) return SD_ERR_CUDA;
@@ -458,7 +460,12 @@ int run_statement(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nb
       dd.positions = mp.out_pos; dd.data = mp.out_vals; dd.nulls = nw ? mp.out_nulls : nullptr;
       dd.n = (int32_t)c.n_union; dd.nwords = nw; dd.enc = ENC_UNCOMPRESSED;
     }
-    if (upd) { d_devd = reinterpret_cast<DevDelta*>(s->arena.alloc(sizeof(DevDelta) * devd.size(), 16)); if (!d_devd) return SD_ERR_CUDA; }
+    if (upd) {
+      d_devd = reinterpret_cast<DevDelta*>(s->arena.alloc(sizeof(DevDelta) * devd.size(), 16));
+      if (!d_devd) return SD_ERR_CUDA;
+      for (int b = 0; b < nb; b++)   // each batch owns its slice of the statement's DevDelta array
+        if (!new_extents[b].empty()) new_extents[b].push_back(Extent{reinterpret_cast<uint8_t*>(d_devd + (size_t)b * T), sizeof(DevDelta) * T});
+    }
   }
   // ---- writing pass ----------------------------------------------------------------------------------------------------
   SD_CUDA(cudaMemcpyAsync(d_pairs, pairs.data(), sizeof(MergePair) * pairs.size(), cudaMemcpyHostToDevice, st));
@@ -477,6 +484,7 @@ int run_statement(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_t nb
     const StoredBatch& old = *ms.batches[b];
     std::unique_ptr<StoredBatch> nbp(new StoredBatch(old));
     nbp->uid = next_batch_uid();
+    nbp->extents.insert(nbp->extents.end(), new_extents[b].begin(), new_extents[b].end());   // (replaced ones pruned at install)
     for (int t = 0; t < T; t++) {
       const size_t i = (size_t)b * T + t;
       const PairCounts& c = counts[i];

@@ -10,6 +10,7 @@
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -152,6 +153,8 @@ uint8_t* Arena::alloc(size_t n, size_t align, size_t misalign) {
       if (off + n <= slabs[cur_slab].bytes) {
         cur_off = off + n;
         used += n;
+        slabs[cur_slab].used += n;
+        if (record) record->push_back(Extent{base + off, n});
         return base + off;
       }
       cur_slab++;
@@ -175,26 +178,38 @@ uint8_t* Arena::alloc(size_t n, size_t align, size_t misalign) {
         set_error(SD_ERR_CUDA, "cudaMalloc(%zu) failed: %s", sz, cudaGetErrorString(e));
         return nullptr;
       }
-      slabs.push_back({(uint8_t*)p, sz, false, false, 0});
+      slabs.push_back({(uint8_t*)p, sz, false, false, 0, 0});
     }
     cur_slab = slabs.size() - 1;
     cur_off = 0;
   }
 }
-void Arena::reset() { cur_slab = 0; cur_off = 0; used = 0; }
-void Arena::release() {
-  if (!slabs.empty()) cudaSetDevice(device);
-  for (auto& s : slabs) {
-    if (s.vmm) {
-      const Vmm& v = vmm();
-      const CUdeviceptr va = reinterpret_cast<CUdeviceptr>(s.base);
-      v.unmap(va, s.bytes);
-      v.release(s.handle);
-      v.address_free(va, s.bytes);
-    } else {
-      cudaFree(s.base);
-    }
+void Arena::reset() {
+  cur_slab = 0; cur_off = 0; used = 0;
+  for (auto& s : slabs) s.used = 0;
+}
+Arena::Slab Arena::detach_slab(size_t i) {
+  const Slab s = slabs[i];
+  used -= s.used;
+  slabs.erase(slabs.begin() + (ptrdiff_t)i);
+  if (cur_slab > i) cur_slab--;
+  else if (cur_slab == i) cur_off = 0;   // (the slab being allocated from: the next allocation moves on)
+  return s;
+}
+void Arena::free_slab(int device, const Slab& s) {
+  cudaSetDevice(device);
+  if (s.vmm) {
+    const Vmm& v = vmm();
+    const CUdeviceptr va = reinterpret_cast<CUdeviceptr>(s.base);
+    v.unmap(va, s.bytes);
+    v.release(s.handle);
+    v.address_free(va, s.bytes);
+  } else {
+    cudaFree(s.base);
   }
+}
+void Arena::release() {
+  for (auto& s : slabs) free_slab(device, s);
   slabs.clear();
   reset();
 }
@@ -619,8 +634,11 @@ int store_install(sd_store* s, FreshBatches& fresh, const std::vector<const Stor
     if (!where.count(f.first)) return set_error(SD_ERR_STATE, "%s: a batch of the snapshot left the store", what);
   for (const StoredBatch* r : remove)
     if (!where.count(r)) return set_error(SD_ERR_STATE, "%s: a batch of the snapshot left the store", what);
+  const int64_t v = s->version + 1;   // snapshots older than this one may still read what leaves the store now
   for (auto& f : fresh) {
     const size_t i = where[f.first];
+    prune_extents(*f.second);
+    s->batches[i]->retired_at = v;
     s->retired.push_back(std::move(s->batches[i]));
     s->batches[i] = std::move(f.second);
   }
@@ -629,13 +647,27 @@ int store_install(sd_store* s, FreshBatches& fresh, const std::vector<const Stor
     for (const StoredBatch* r : remove) drop[where[r]] = true;
     size_t k = 0;
     for (size_t i = 0; i < s->batches.size(); i++) {
-      if (drop[i]) s->retired.push_back(std::move(s->batches[i]));
+      if (drop[i]) { s->batches[i]->retired_at = v; s->retired.push_back(std::move(s->batches[i])); }
       else s->batches[k++] = std::move(s->batches[i]);
     }
     s->batches.resize(k);
   }
-  s->version++;
+  s->version = v;
   return 0;
+}
+
+void prune_extents(StoredBatch& b) {
+  std::vector<Extent>& e = b.extents;
+  std::sort(e.begin(), e.end(), [](const Extent& x, const Extent& y) { return x.ptr < y.ptr; });
+  std::vector<char> used(e.size(), 0);
+  visit_device_pointers(b, [&](uintptr_t a, int, const char*) {
+    auto it = std::upper_bound(e.begin(), e.end(), a, [](uintptr_t x, const Extent& y) { return x < (uintptr_t)y.ptr; });
+    if (it != e.begin() && a < (uintptr_t)(it - 1)->ptr + (it - 1)->bytes) used[(size_t)(it - e.begin() - 1)] = 1;
+    return a;
+  });
+  size_t k = 0;
+  for (size_t i = 0; i < e.size(); i++) if (used[i]) e[k++] = e[i];
+  e.resize(k);
 }
 
 int store_register_encoded(sd_store* s, const uint8_t* prefix, int64_t prefix_len, int64_t total_len, int type, int nullable,
@@ -710,6 +742,7 @@ int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals) {
   std::unique_ptr<StoredBatch> sb(new StoredBatch());
   sb->num_rows = b->num_rows; sb->bucket_id = b->bucket_id; sb->batch_id = b->batch_id;
   sb->cols.resize(s->schema.size());
+  ExtentRecorder rec(s->arena, &sb->extents);   // every arena allocation of this put belongs to the new batch
   {   // LZ4 envelopes that lie (almost) back to back in host memory: one host->device copy for the lot (small copies reach
       // a lower link rate than large ones)
     s->span_h0 = nullptr;
@@ -874,6 +907,10 @@ int sd_store_create(int device, int32_t ncols, const sd_column* schema, sd_store
   s->device = device;
   s->arena.device = device;
   s->arena.compressible = true;
+  if (const char* env = getenv("SD_TUNE_STORE_SLAB_MB")) {   // (tests: stores of many small slabs)
+    const long v = atol(env);
+    if (v >= 2 && v <= 4096) s->arena.slab_bytes = size_t(v) << 20;
+  }
   s->lz4_stage.device = device;
   s->lz4_stage.slab_bytes = size_t(256) << 20;
   s->schema.assign(schema, schema + ncols);
