@@ -45,8 +45,13 @@ typedef enum sd_type {
   SD_DATE = 8,       /* int32 days since epoch       */
   SD_TIMESTAMP = 9,  /* int64 microseconds           */
   SD_STRING = 10,    /* UTF8String                   */
-  SD_DECIMAL = 11    /* column values: precision <= 18, int64 unscaled (enc/Uncompressed.scala:95-98); aggregate
-                        buffers / results may be wider (SUM: DECIMAL(p+10,s), up to 128-bit unscaled), see sd_agg */
+  SD_DECIMAL = 11    /* column values: precision <= 18, int64 unscaled (enc/Uncompressed.scala:95-98); precision 19..38,
+                        back-to-back [int32 len][BigInteger.toByteArray() of the unscaled value, 1..16 bytes]
+                        (enc/Uncompressed.scala:330-345).  A "wide" DECIMAL (precision > 18) is read, compared, cast up,
+                        tested with IN / IS [NOT] NULL, grouped and aggregated; arithmetic on it, casts from it to anything
+                        but an equal or wider DECIMAL, startsWith and SET values of that type are SD_ERR_UNSUPPORTED; it is
+                        refused in update deltas, sd_store_encode_batch and sd_store_compact.  Aggregate buffers / results
+                        may be wider (SUM: DECIMAL(min(38,p+10),s)), see sd_agg */
 } sd_type;
 
 /* One projected scan column (ColumnTableScan.output attribute). */
@@ -56,7 +61,7 @@ typedef struct sd_column {
                              (enc/ColumnEncoding.scala:817-822)                       */
   int32_t table_ordinal;  /* 0-based column of the table (ColumnFormatKey.columnIndex-1) */
   int32_t scale;          /* SD_DECIMAL scale; else 0                                 */
-  int32_t precision;      /* SD_DECIMAL precision (1..18 for a scan column); else 0   */
+  int32_t precision;      /* SD_DECIMAL precision (1..38 for a scan column); else 0   */
 } sd_column;
 
 /* Expression tree, flattened; children always precede parents.  Mirrors the Catalyst trees that
@@ -103,7 +108,11 @@ typedef struct sd_expr {
  * DECIMAL(p,s) input (Spark 2.1.1 Sum / Average): SUM buffer and result DECIMAL(p+10,s); AVG buffers
  * [sum DECIMAL(p+10,s), count LONG], result DECIMAL(p+4,s+4) = sum / count rounded HALF_UP.  In UnsafeRows a DECIMAL
  * of precision <= 18 is its unscaled int64 in the fixed slot; wider ones are (offset << 32 | size) + the
- * BigInteger two's-complement big-endian bytes in a 16-byte reserved region (UnsafeRowWriter.write(Decimal)). */
+ * BigInteger two's-complement big-endian bytes in a 16-byte reserved region (UnsafeRowWriter.write(Decimal)).
+ * Wide DECIMAL input (precision > 18): SUM / AVG sum each value as four 32-bit limbs (exact below 2^31 rows per execution),
+ * a total of more than min(38, p+10) digits is NULL -- in partial rows such a total is written as 10^(buffer precision), a
+ * value no in-range total reaches, and the merges keep it so (they add partial totals exactly); MIN / MAX keep the input type; AVG's result is
+ * DECIMAL(min(38,p+4), min(38,s+4)) rounded HALF_UP, NULL when it does not fit. */
 typedef enum sd_agg_fn {
   SD_AGG_COUNT_STAR = 1, SD_AGG_COUNT = 2, SD_AGG_SUM = 3, SD_AGG_AVG = 4, SD_AGG_MIN = 5, SD_AGG_MAX = 6
 } sd_agg_fn;
@@ -133,7 +142,8 @@ typedef struct sd_plan_desc {
 typedef struct sd_literal {
   int32_t type;      /* sd_type                              */
   int32_t is_null;
-  int64_t i;         /* integral / date / timestamp / boolean / decimal-unscaled value */
+  int64_t i;         /* integral / date / timestamp / boolean / decimal-unscaled value (ignored for a DECIMAL slot
+                        of precision > 18, whose unscaled value is BigInteger.toByteArray() bytes in s / slen) */
   double  d;         /* FLOAT / DOUBLE value                 */
   const char* s;     /* STRING bytes (not NUL terminated)    */
   int32_t slen;

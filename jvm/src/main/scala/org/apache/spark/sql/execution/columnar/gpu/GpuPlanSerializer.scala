@@ -84,7 +84,8 @@ object GpuPlanSerializer {
     case IntegerType => Some(Abi.INT); case LongType => Some(Abi.LONG); case FloatType => Some(Abi.FLOAT)
     case DoubleType => Some(Abi.DOUBLE); case DateType => Some(Abi.DATE); case TimestampType => Some(Abi.TIMESTAMP)
     case StringType => Some(Abi.STRING)
-    case d: DecimalType if d.precision <= Decimal.MAX_LONG_DIGITS => Some(Abi.DECIMAL)   // int64 unscaled (enc/Uncompressed.scala:95-98)
+    // precision <= 18: int64 unscaled (enc/Uncompressed.scala:95-98); wider: [len][BigInteger bytes] records (:330-345)
+    case _: DecimalType => Some(Abi.DECIMAL)
     case _ => None
   }
   private def decPS(dt: DataType): Int = dt match {
@@ -257,7 +258,8 @@ object GpuPlanSerializer {
     base
   }
 
-  /** sd_literal[n] for this execution: {type:4, is_null:4, i:8, d:8, s:8, slen:4, pad:4}; string bytes follow the array */
+  /** sd_literal[n] for this execution: {type:4, is_null:4, i:8, d:8, s:8, slen:4, pad:4}; string bytes follow the array, and
+   *  so do the unscaled values of DECIMAL slots wider than 18 digits (BigInteger.toByteArray at the slot's scale) */
   def writeLiterals(literals: Array[LiteralSlot]): NativeBlock = {
     val values = literals.map { l =>
       l.expr match {
@@ -268,6 +270,11 @@ object GpuPlanSerializer {
     }
     val strings = values.zip(literals).map {
       case (s: UTF8String, l) if !l.stringAsDate => s.getBytes
+      case (v: Decimal, l) => l.expr.dataType match {
+        case d: DecimalType if d.precision > Decimal.MAX_LONG_DIGITS =>
+          v.toJavaBigDecimal.setScale(d.scale).unscaledValue.toByteArray
+        case _ => null
+      }
       case _ => null
     }
     val head = literals.length.toLong * Abi.SIZEOF_LITERAL
@@ -297,6 +304,11 @@ object GpuPlanSerializer {
         case v: Long => Platform.putLong(null, o + 8, v)                // LONG and TIMESTAMP
         case v: Float => Platform.putDouble(null, o + 16, v.toDouble)
         case v: Double => Platform.putDouble(null, o + 16, v)
+        case _: Decimal if strings(i) ne null =>         // DECIMAL(p > 18): its bytes, like a string literal's
+          val bytes = strings(i)
+          Platform.copyMemory(bytes, Platform.BYTE_ARRAY_OFFSET, null, tail, bytes.length)
+          Platform.putLong(null, o + 24, tail); Platform.putInt(null, o + 32, bytes.length)
+          tail += bytes.length
         case v: Decimal => Platform.putLong(null, o + 8, v.toUnscaledLong)   // at the slot's scale (Catalyst cast it to the column type)
         case other => throw new IllegalStateException(s"literal value $other of ${other.getClass}")
       }

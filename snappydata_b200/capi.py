@@ -13,7 +13,7 @@ from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from .column_format import ColumnBatch, SqlType, parse_row_stream
+from .column_format import ColumnBatch, SqlType, decimal_bytes, parse_row_stream
 
 SD_ABI_VERSION = 2
 SD_NUM_METRICS = 12
@@ -151,14 +151,19 @@ class MarshalledBatch:
         self.c = b
 
 
-def make_literal(t: SqlType, v) -> sd_literal:
+def make_literal(t: SqlType, v, wide: bool = False) -> sd_literal:
+    """`wide`: the slot holds a DECIMAL of more than 18 digits; an int value is passed as its BigInteger bytes."""
     lit = sd_literal()
     lit.type = int(t)
     if v is None:
         lit.is_null = 1
         return lit
     t = SqlType(t)
-    if t == SqlType.STRING:
+    if wide:
+        b = bytes(v) if isinstance(v, (bytes, bytearray)) else decimal_bytes(int(v))
+        lit.s = b
+        lit.slen = len(b)
+    elif t == SqlType.STRING:
         b = v if isinstance(v, bytes) else str(v).encode("utf-8")
         lit.s = b
         lit.slen = len(b)
@@ -299,6 +304,14 @@ class PlanDesc:
         self.proj_py = list(proj)
         self.literal_types_py = [SqlType(t) for t in literal_types]
         self.filter = filter_node
+        # literal slots of a DECIMAL wider than 18 digits: a LIT node of that type, or an IN list over such an operand
+        self.lit_wide = [False] * len(self.literal_types_py)
+        for i, (op, t, a, b, c) in enumerate(self.exprs_py):
+            if op == Op.LIT and self._wide(i):
+                self.lit_wide[a] = True
+            if op == Op.IN and self._wide(a):
+                for k in range(c):
+                    self.lit_wide[b + k] = True
         self._cols = (sd_column * max(1, len(self.cols_py)))()
         for i, c in enumerate(self.cols_py):
             self._cols[i] = sd_column(int(c[0]), int(bool(c[1])), int(c[2]), int(c[3]) if len(c) > 3 else 0,
@@ -339,6 +352,9 @@ class PlanDesc:
         if op == Op.NEG:
             return self._ps(a)
         return c >> 8, c & 0xFF
+
+    def _wide(self, node: int) -> bool:
+        return SqlType(self.exprs_py[node][1]) == SqlType.DECIMAL and self._ps(node)[0] > 18
 
     def _ftype(self, node: int):
         t = SqlType(self.exprs_py[node][1])
@@ -399,7 +415,7 @@ class Plan:
         n = len(values)
         arr = (sd_literal * max(1, n))()
         for i, v in enumerate(values):
-            arr[i] = make_literal(self.desc.literal_types_py[i], v)
+            arr[i] = make_literal(self.desc.literal_types_py[i], v, self.desc.lit_wide[i])
         return arr
 
     def set_literals(self, values: Sequence[object]):
@@ -636,12 +652,15 @@ class Store:
     """Device-resident column store handle (product only)."""
 
     def __init__(self, api: Api, schema, device: int = 0):
-        """schema: [(SqlType, nullable)] per table column, in table order."""
+        """schema: [(SqlType, nullable[, precision, scale])] per table column, in table order (DECIMAL precision
+        defaults to 18)."""
         self.api = api
-        self.schema = [(SqlType(t), bool(n)) for t, n in schema]
+        self.schema = [(SqlType(c[0]), bool(c[1])) for c in schema]
         arr = (sd_column * max(1, len(self.schema)))()
-        for i, (t, n) in enumerate(self.schema):
-            arr[i] = sd_column(int(t), int(n), i, 0, 18 if int(t) == int(SqlType.DECIMAL) else 0)
+        for i, c in enumerate(schema):
+            t, n = int(c[0]), int(bool(c[1]))
+            prec, scale = (int(c[2]), int(c[3])) if len(c) > 3 else (18 if t == int(SqlType.DECIMAL) else 0, 0)
+            arr[i] = sd_column(t, n, i, scale, prec)
         h = C.c_void_p()
         api.check(api.store_create(device, len(self.schema), arr, C.byref(h)))
         self.h = h

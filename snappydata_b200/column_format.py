@@ -124,6 +124,28 @@ def encode_uncompressed(values, sql_type: SqlType, nulls=None) -> bytes:
     return _header(UNCOMPRESSED, nw) + arr.tobytes()
 
 
+def decimal_bytes(unscaled: int) -> bytes:
+    """BigInteger.toByteArray(): the minimal big-endian two's complement of an unscaled DECIMAL value."""
+    n = (int(unscaled) + (unscaled < 0)).bit_length() // 8 + 1
+    return int(unscaled).to_bytes(n, "big", signed=True)
+
+
+def encode_wide_decimal(values, nulls=None) -> bytes:
+    """typeId 0 for DECIMAL(p > 18): back-to-back [int32 len][BigInteger bytes] of the non-null unscaled values
+    (enc/Uncompressed.scala:330-345)."""
+    nw = null_words(nulls)
+    vals = [int(v) for i, v in enumerate(values) if nulls is None or not nulls[i]]
+    return _header(UNCOMPRESSED, nw) + b"".join(struct.pack("<i", len(decimal_bytes(v))) + decimal_bytes(v) for v in vals)
+
+
+def wide_decimal_stats(values, precision: int, scale: int, nulls=None):
+    """column_stats for DECIMAL(p > 18): bounds are unscaled ints, typed (DECIMAL, precision, scale) for the stats row."""
+    vals = [int(v) for i, v in enumerate(values) if nulls is None or not nulls[i]]
+    nc = int(np.count_nonzero(nulls)) if nulls is not None else 0
+    t = (SqlType.DECIMAL, precision, scale)
+    return (t, min(vals), max(vals), nc) if vals else (t, None, None, nc)
+
+
 def _b(v) -> bytes:
     return v if isinstance(v, (bytes, bytearray, np.bytes_)) else str(v).encode("utf-8")
 
@@ -273,12 +295,17 @@ def unsafe_row(fields: Sequence[Tuple[SqlType, object]]) -> bytes:
     var = bytearray()
     fixed_len = len(bitset) + len(slots)
     for i, (t, v) in enumerate(fields):
-        t = SqlType(t)
+        wide = isinstance(t, tuple) and t[1] > 18   # (DECIMAL, precision, scale): BigInteger bytes in a 16-byte region
+        t = SqlType(t[0] if isinstance(t, tuple) else t)
         if v is None:
             bitset[i >> 3] |= 1 << (i & 7)
             continue
         off = 8 * i
-        if t == SqlType.STRING:
+        if wide:
+            b = decimal_bytes(v)
+            struct.pack_into("<q", slots, off, ((fixed_len + len(var)) << 32) | len(b))
+            var += b + b"\0" * (16 - len(b))
+        elif t == SqlType.STRING:
             b = _b(v)
             struct.pack_into("<q", slots, off, ((fixed_len + len(var)) << 32) | len(b))
             var += b + b"\0" * ((-len(b)) % 8)

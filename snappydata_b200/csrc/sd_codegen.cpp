@@ -31,6 +31,11 @@ int decimal_ps(const PlanSpec& p, int node) {
   if (e.op == SD_OP_NEG) return decimal_ps(p, e.a);
   return e.c;
 }
+bool node_is_wide(const PlanSpec& p, int node) {
+  return p.exprs[node].type == SD_DECIMAL && (decimal_ps(p, node) >> 8) > 18;
+}
+int kind_of_column(const sd_column& c) { return wide_decimal(c.type, c.precision) ? K_CODE : kind_of_type(c.type); }
+static const char* col_ctype(const sd_column& c);
 std::vector<int> partial_field_types(const PlanSpec& p) {
   std::vector<int> t;
   for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
@@ -78,6 +83,7 @@ static const char* ctype_of(int t) {
   }
   return "void";
 }
+static const char* col_ctype(const sd_column& c) { return wide_decimal(c.type, c.precision) ? "int32_t" : ctype_of(c.type); }
 static const char* tname(int t) {
   static const char* n[] = {"?", "bool", "i8", "i16", "i32", "i64", "f32", "f64", "date", "ts", "str", "dec"};
   return (t >= 1 && t <= 11) ? n[t] : "?";
@@ -195,8 +201,8 @@ struct Gen {
     if ((int)p.cols.size() > 64) return fail(SD_ERR_UNSUPPORTED, "more than 64 scan columns in one fused plan");
     if ((int)p.literal_types.size() > MAX_LITERALS) return fail(SD_ERR_UNSUPPORTED, "more than 64 literal slots");
     for (auto& c : p.cols) if (kind_of_type(c.type) < 0) return fail(SD_ERR_INVALID, "unknown column type");
-    for (auto& c : p.cols) if (c.type == SD_DECIMAL && (c.precision < 1 || c.precision > 18 || c.scale < 0 || c.scale > c.precision))
-      return fail(SD_ERR_INVALID, "DECIMAL scan column needs 1 <= precision <= 18 (int64 unscaled values, enc/Uncompressed.scala:95-98)");
+    for (auto& c : p.cols) if (c.type == SD_DECIMAL && (c.precision < 1 || c.precision > 38 || c.scale < 0 || c.scale > c.precision))
+      return fail(SD_ERR_INVALID, "DECIMAL scan column needs 1 <= precision <= 38 and 0 <= scale <= precision");
     for (int i = 0; i < ne; i++) {
       const sd_expr& e = p.exprs[i];
       if (e.op == SD_OP_COL) { if (e.a < 0 || e.a >= (int)p.cols.size()) return fail(SD_ERR_INVALID, "column reference out of range"); }
@@ -209,8 +215,19 @@ struct Gen {
       if (kind_of_type(e.type) < 0) return fail(SD_ERR_INVALID, "unknown expression type");
       if (e.type == SD_DECIMAL) {
         const int ps = decimal_ps(p, i), pr = ps >> 8, sc = ps & 0xff;
-        if (pr < 1 || pr > 18 || sc > pr) return fail(SD_ERR_INVALID, "DECIMAL expression needs 1 <= precision <= 18 and scale <= precision (sd_expr.c / sd_column)");
+        if (pr < 1 || pr > 38 || sc > pr) return fail(SD_ERR_INVALID, "DECIMAL expression needs 1 <= precision <= 38 and scale <= precision (sd_expr.c / sd_column)");
       }
+      // DECIMAL wider than 18 digits: read, compared, cast up, grouped and aggregated; no arithmetic on it
+      const bool wide_here = node_is_wide(p, i);
+      const bool wide_a = e.op != SD_OP_COL && e.op != SD_OP_LIT && node_is_wide(p, e.a);
+      const bool wide_b = e.op != SD_OP_COL && e.op != SD_OP_LIT && !is_unary(e.op) && node_is_wide(p, e.b);
+      if ((e.op >= SD_OP_ADD && e.op <= SD_OP_NEG) && (wide_here || wide_a || wide_b))
+        return fail(SD_ERR_UNSUPPORTED, "arithmetic on a DECIMAL wider than 18 digits");
+      if (e.op == SD_OP_STARTSWITH && (wide_a || wide_b)) return fail(SD_ERR_UNSUPPORTED, "startsWith on a DECIMAL wider than 18 digits");
+      if (e.op == SD_OP_CAST && wide_a && !(wide_here && (decimal_ps(p, i) & 0xff) >= (decimal_ps(p, e.a) & 0xff)))
+        return fail(SD_ERR_UNSUPPORTED, "cast from a DECIMAL wider than 18 digits to anything but an equal or wider DECIMAL");
+      if (e.op == SD_OP_CAST && wide_here && !wide_a && p.exprs[e.a].type != SD_DECIMAL)
+        return fail(SD_ERR_UNSUPPORTED, "cast to a DECIMAL wider than 18 digits from a non-DECIMAL type");
       if (e.op == SD_OP_CAST) {   // refused casts are refused at plan creation, whether or not the node ends up in generated code
         const int from = p.exprs[e.a].type, to = e.type;
         const bool tf = from == SD_DATE || from == SD_TIMESTAMP, tt = to == SD_DATE || to == SD_TIMESTAMP;
@@ -287,6 +304,7 @@ struct Gen {
       AggMap m;
       memset(&m, 0, sizeof(m));
       m.fn = a.fn; m.value_slot = -1; m.count_slot = -1;
+      for (int& l : m.limb_slot) l = -1;
       const int it = a.expr >= 0 ? p.exprs[a.expr].type : SD_LONG;
       const int in_null = a.expr >= 0 ? static_nullable(a.expr) : 0;
       m.in_type = it;
@@ -312,6 +330,27 @@ struct Gen {
       if (it == SD_DECIMAL) {
         m.in_ps = decimal_ps(p, a.expr);
         m.buf_ps = m.in_ps;   // MIN / MAX keep the input type
+      }
+      if ((a.fn == SD_AGG_MIN || a.fn == SD_AGG_MAX) && node_is_wide(p, a.expr)) {
+        // the slot holds the address of the winning value's record, compared by value
+        if (p.exprs[a.expr].op != SD_OP_COL) return fail(SD_ERR_UNSUPPORTED, "MIN / MAX of a wide DECIMAL expression that is not a column");
+        m.buf_type = SD_DECIMAL;
+        m.value_slot = add_slot(a.fn == SD_AGG_MIN ? SLOT_MIN_DEC : SLOT_MAX_DEC, a.expr, GATE_DECREF);
+        m.buf_nullable = keyed ? in_null : 1;
+        if (m.buf_nullable) m.count_slot = count_slot_for(a.expr);
+        p.agg_map.push_back(m);
+        continue;
+      }
+      if ((a.fn == SD_AGG_SUM || a.fn == SD_AGG_AVG) && node_is_wide(p, a.expr)) {
+        // buffer DECIMAL(min(38, p + 10), s); the value is summed as four 32-bit limbs, recombined on the host
+        m.buf_type = SD_DECIMAL;
+        m.buf_ps = (std::min(38, (m.in_ps >> 8) + 10) << 8) | (m.in_ps & 0xff);
+        for (int l = 0; l < 4; l++) m.limb_slot[l] = add_slot(SLOT_ADD_I64, a.expr, GATE_LIMB0 + l);
+        m.value_slot = m.limb_slot[3];
+        if (a.fn == SD_AGG_SUM) { m.buf_nullable = keyed ? in_null : 1; if (m.buf_nullable) m.count_slot = count_slot_for(a.expr); }
+        else m.count_slot = count_slot_for(a.expr);
+        p.agg_map.push_back(m);
+        continue;
       }
       if ((a.fn == SD_AGG_SUM || a.fn == SD_AGG_AVG) && it == SD_DECIMAL) {
         // Spark 2.1.1 Sum / Average over DECIMAL(p,s): buffer DECIMAL(p+10,s) -- up to 28 digits, i.e. wider than int64.
@@ -376,18 +415,30 @@ struct Gen {
     }
     done[node] = 1;
     const std::string N = std::to_string(node);
-    const char* T = ctype_of(e.type);
+    const bool wide = node_is_wide(p, node);
+    const char* T = wide ? "sd::i128" : ctype_of(e.type);
     auto V = [&](int n) { return "v" + std::to_string(n); };
     auto NL = [&](int n) { return "n" + std::to_string(n); };
     auto finish_bool = [&]() { o << "    const bool n" << N << " = t" << N << " == 2; const uint8_t v" << N << " = t" << N << " == 1;\n"; };
     switch (e.op) {
       case SD_OP_COL:
+        if (wide) {   // the row holds the position of the value's record in the batch body
+          const std::string C = std::to_string(e.a), nl = p.cols[e.a].nullable ? "r.n" + C : std::string("false");
+          o << "    const bool n" << N << " = " << nl << "; const sd::i128 v" << N << " = n" << N
+            << " ? (sd::i128)0 : sd::dec_rec(ctx.strbase[" << C << "] + (uint32_t)r.c" << C << ");\n";
+          return 0;
+        }
         o << "    const " << T << " v" << N << " = r.c" << e.a << "; const bool n" << N << " = "
           << (p.cols[e.a].nullable ? "r.n" + std::to_string(e.a) : std::string("false")) << ";\n";
         if (e.type == SD_BOOLEAN) o << "    const int t" << N << " = n" << N << " ? 2 : (v" << N << " ? 1 : 0);\n";
         return 0;
       case SD_OP_LIT: {
         if (e.type == SD_STRING) { o << "    const int32_t v" << N << " = 0; const bool n" << N << " = false;\n"; return 0; }
+        if (wide) {
+          o << "    const sd::i128 v" << N << " = sd::dec_lit(ctx.lit_bytes(" << e.a << ")); const bool n" << N << " = "
+            << (p.lit_nullable ? "((ctx.L->nullmask >> " + std::to_string(e.a) + ") & 1ull) != 0" : std::string("false")) << ";\n";
+          return 0;
+        }
         std::string val = type_is_fp(e.type) ? "ctx.L->d[" + std::to_string(e.a) + "]" : "ctx.L->i[" + std::to_string(e.a) + "]";
         if (e.type == SD_BOOLEAN) val = "(" + val + " != 0)";
         o << "    const " << T << " v" << N << " = (" << T << ")" << val << "; const bool n" << N << " = "
@@ -424,6 +475,14 @@ struct Gen {
         auto pow10 = [](int k) { std::string r = "1"; for (int i = 0; i < k; i++) r += "0"; return r + "ll"; };
         if (from == SD_STRING || to == SD_STRING) return fail(SD_ERR_UNSUPPORTED, "casts involving STRING");
         if ((is_time(from) || is_time(to)) && from != to) return fail(SD_ERR_UNSUPPORTED, "casts involving DATE / TIMESTAMP (time-zone dependent in Spark)");
+        if (wide) {   // DECIMAL(p1, s1) -> DECIMAL(p2 > 18, s2 >= s1) in 128 bits, NULL when it does not fit p2 digits
+          const int ps0 = decimal_ps(p, e.a), ps1 = decimal_ps(p, node);
+          const int up = (ps1 & 0xff) - (ps0 & 0xff), k = (ps1 >> 8) - up;
+          const std::string a = "(sd::i128)" + V(e.a);
+          o << "    const sd::i128 v" << N << " = (sd::i128)((unsigned __int128)" << a << " * (unsigned __int128)sd::p10w(" << up << ")); const bool n" << N
+            << " = " << NL(e.a) << " || " << a << " >= sd::p10w(" << k << ") || " << a << " <= -sd::p10w(" << k << ");\n";
+          return 0;
+        }
         if (from == SD_DECIMAL || to == SD_DECIMAL) {
           if (from == SD_DECIMAL && type_is_fp(to)) {   // Decimal.toDouble: unscaled / 10^s
             const int sc = decimal_ps(p, e.a) & 0xff;
@@ -500,6 +559,7 @@ struct Gen {
             const int s = e.b + k;
             std::string lv = type_is_fp(ot) ? std::string("(") + ctype_of(ot) + ")ctx.L->d[" + std::to_string(s) + "]"
                                             : std::string("(") + ctype_of(ot) + ")ctx.L->i[" + std::to_string(s) + "]";
+            if (node_is_wide(p, e.a)) lv = "sd::dec_lit(ctx.lit_bytes(" + std::to_string(s) + "))";
             std::string nn = p.lit_nullable ? "(((ctx.L->nullmask >> " + std::to_string(s) + ") & 1ull) == 0)" : std::string("true");
             std::string eq = type_is_fp(ot) ? "sd::f_eq(" + V(e.a) + ", " + lv + ")" : "(" + V(e.a) + " == " + lv + ")";
             any << (k ? " || " : "") << "(" << nn << " && " << eq << ")";
@@ -583,6 +643,13 @@ struct Gen {
       for (size_t j = 0; j < p.proj.size(); j++) {
         const sd_expr& e = p.exprs[p.proj[j]];
         sig << (j ? "," : "") << expr_text(p, p.proj[j]);
+        if (node_is_wide(p, p.proj[j])) {   // a wide DECIMAL column: the device address of its record (the host reads the bytes)
+          const std::string C = std::to_string(e.a);
+          projfn << "    pv[" << j << "] = (uint64_t)(uintptr_t)(ctx.strbase[" << C << "] + (uint32_t)r.c" << C << ");";
+          if (p.cols[e.a].nullable) projfn << " if (r.n" << C << ") pnull |= " << (1u << j) << "u;";
+          projfn << "\n";
+          continue;
+        }
         int rc = emit_node(p.proj[j], done, projfn);
         if (rc) return rc;
         const std::string N = std::to_string(p.proj[j]);
@@ -602,6 +669,10 @@ struct Gen {
           strkeymask |= 1u << k;
           if (p.cols[e.a].nullable) keyfn << "    if (r.n" << e.a << ") { knull |= " << (1u << k) << "u; kc[" << k << "] = 0; } else";
           keyfn << "    kc[" << k << "] = ctx.str_ref(" << e.a << ", " << t << ", r.c" << e.a << ");\n";
+        } else if (node_is_wide(p, p.keys[k])) {   // by reference like a string: equal values have identical bytes
+          strkeymask |= 1u << k;
+          if (p.cols[e.a].nullable) keyfn << "    if (r.n" << e.a << ") { knull |= " << (1u << k) << "u; kc[" << k << "] = 0; } else";
+          keyfn << "    kc[" << k << "] = (int64_t)(uintptr_t)(ctx.strbase[" << e.a << "] + (uint32_t)r.c" << e.a << ");\n";
         } else {
           int rc = emit_node(p.keys[k], done, keyfn);
           if (rc) return rc;
@@ -621,7 +692,7 @@ struct Gen {
     for (size_t s = 0; s < p.slots.size(); s++) {
       const SlotSpec& x = p.slots[s];
       sig << (s ? "," : "") << x.op << "/" << x.gate << "/" << (x.node >= 0 ? expr_text(p, x.node) : std::string("-"));
-      if (x.node >= 0) { int rc = emit_node(x.node, done, slt); if (rc) return rc; }
+      if (x.node >= 0 && x.gate != GATE_DECREF) { int rc = emit_node(x.node, done, slt); if (rc) return rc; }
       const std::string V = "v" + std::to_string(x.node), NL = "n" + std::to_string(x.node);
       slt << "    sv[" << s << "] = ";
       if (x.gate == GATE_ONE) slt << "1ull;\n";
@@ -630,6 +701,13 @@ struct Gen {
         const int col = p.exprs[x.node].a;
         slt << NL << " ? 0ull : (uint64_t)ctx.str_ref(" << col << ", " << x.table << ", r.c" << col << ");\n";
       }
+      else if (x.gate == GATE_DECREF) {
+        const std::string C = std::to_string(p.exprs[x.node].a);
+        slt << (p.cols[p.exprs[x.node].a].nullable ? "r.n" + C : std::string("false")) << " ? 0ull : (uint64_t)(uintptr_t)(ctx.strbase[" << C << "] + (uint32_t)r.c" << C << ");\n";
+      }
+      else if (x.gate == GATE_LIMB3) slt << NL << " ? 0ull : (uint64_t)(int64_t)(" << V << " >> 96);\n";
+      else if (x.gate >= GATE_LIMB0 && x.gate <= GATE_LIMB2)
+        slt << NL << " ? 0ull : (uint64_t)(uint32_t)((unsigned __int128)" << V << " >> " << 32 * (x.gate - GATE_LIMB0) << ");\n";
       else if (x.gate == GATE_VALUE_HI32) slt << NL << " ? 0ull : (uint64_t)((int64_t)" << V << " >> 32);\n";
       else if (x.gate == GATE_VALUE_LO32) slt << NL << " ? 0ull : ((uint64_t)(int64_t)" << V << " & 0xffffffffull);\n";
       else {
@@ -668,7 +746,12 @@ struct Gen {
     o << "  static constexpr bool SLOW_PATHS = " << (p.slow_paths ? "true" : "false") << ";\n";
     o << "  static constexpr int NTABLES = " << p.tables.size() << ";\n";
     o << "  static constexpr unsigned STRKEYMASK = " << strkeymask << "u;\n";
-    { bool anys = false; for (auto& c : p.cols) anys = anys || c.type == SD_STRING; o << "  static constexpr bool ANY_STRING = " << (anys ? "true" : "false") << ";\n"; }
+    for (auto& x : p.slots)
+      if (x.op == SLOT_MIN_DEC || x.op == SLOT_MAX_DEC) {   // slot_combine compares these by value only with 128-bit integers
+        o << "  static_assert(sd::HAVE_I128, \"MIN / MAX of a wide DECIMAL needs 128-bit integers (NVRTC -device-int128)\");\n";
+        break;
+      }
+    { bool anys = false; for (auto& c : p.cols) anys = anys || c.type == SD_STRING || wide_decimal(c.type, c.precision); o << "  static constexpr bool ANY_STRING = " << (anys ? "true" : "false") << ";\n"; }
     o << "  __host__ __device__ static constexpr int kind(int c) { return ";
     for (int c = 0; c < nc; c++) o << "c == " << c << " ? " << p.kinds[c] << " : ";
     o << "0; }\n";
@@ -684,9 +767,9 @@ struct Gen {
     o << "0; }\n";
     o << "  __device__ static __forceinline__ int slot_op_rt(int s) { return slot_op(s); }\n";
     o << "  struct Row {\n";
-    for (int c = 0; c < nc; c++) o << "    " << ctype_of(p.cols[c].type) << " c" << c << "; bool n" << c << ";\n";
+    for (int c = 0; c < nc; c++) o << "    " << col_ctype(p.cols[c]) << " c" << c << "; bool n" << c << ";\n";
     o << "    template <int C, class T> __device__ __forceinline__ void set(T v, bool isnull) {\n";
-    for (int c = 0; c < nc; c++) o << "      if (C == " << c << ") { c" << c << " = (" << ctype_of(p.cols[c].type) << ")v; n" << c << " = isnull; }\n";
+    for (int c = 0; c < nc; c++) o << "      if (C == " << c << ") { c" << c << " = (" << col_ctype(p.cols[c]) << ")v; n" << c << " = isnull; }\n";
     o << "    }\n  };\n";
     o << "  __device__ static __forceinline__ bool filter(const Row& r, const sd::RowCtx& ctx) {\n" << filt.str() << "  }\n";
     o << "  __device__ static __forceinline__ int group(const Row& r, const sd::RowCtx& ctx) {\n" << grp.str() << "  }\n";
@@ -720,7 +803,13 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
   Gen g(out, err);
   int rc = g.validate();
   if (rc) return rc;
-  for (auto& c : out.cols) out.kinds.push_back(kind_of_type(c.type));
+  for (auto& c : out.cols) out.kinds.push_back(kind_of_column(c));
+  out.lit_wide.assign(out.literal_types.size(), 0);   // slots read by a wide LIT node or listed by an IN over a wide operand
+  for (size_t i = 0; i < out.exprs.size(); i++) {
+    const sd_expr& e = out.exprs[i];
+    if (e.op == SD_OP_LIT && node_is_wide(out, (int)i)) out.lit_wide[(size_t)e.a] = 1;
+    if (e.op == SD_OP_IN && node_is_wide(out, e.a)) for (int k = 0; k < e.c; k++) out.lit_wide[(size_t)(e.b + k)] = 1;
+  }
   g.nullability();
   const bool projection = out.aggs.empty() && out.keys.empty();
   if (mutate && !projection) { err = "an UPDATE / DELETE plan has no grouping keys and no aggregates"; return SD_ERR_INVALID; }
@@ -730,6 +819,8 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
     for (int n : out.proj) {
       const sd_expr& e = out.exprs[n];
       if (e.type == SD_STRING && e.op != SD_OP_COL) { err = "projected STRING expression that is not a dictionary column"; return SD_ERR_UNSUPPORTED; }
+      if (node_is_wide(out, n) && mutate) { err = "UPDATE with a SET value that is a DECIMAL wider than 18 digits"; return SD_ERR_UNSUPPORTED; }
+      if (node_is_wide(out, n) && e.op != SD_OP_COL) { err = "projected wide DECIMAL expression that is not a column"; return SD_ERR_UNSUPPORTED; }
     }
   }
   out.mode = mutate ? MODE_MUTATE : projection ? MODE_PROJECT : MODE_NOKEY;
@@ -739,6 +830,7 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
       const sd_expr& e = out.exprs[k];
       if (!(e.op == SD_OP_COL && e.type == SD_STRING)) all_dict_strings = false;
       if (e.type == SD_STRING && e.op != SD_OP_COL) { err = "STRING group key that is not a dictionary column"; return SD_ERR_UNSUPPORTED; }
+      if (node_is_wide(out, k) && e.op != SD_OP_COL) { err = "wide DECIMAL group key that is not a column"; return SD_ERR_UNSUPPORTED; }
     }
     // dense table: <= 4 dictionary-string keys; anything else (other key types, more keys) goes through the hash table
     out.mode = (all_dict_strings && (int)out.keys.size() <= MAX_KEYS && !(opt && opt->force_hash)) ? MODE_GROUPS : MODE_HASH;

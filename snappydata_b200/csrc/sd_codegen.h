@@ -25,7 +25,11 @@ struct TableSpec {
 // GATE_VALUE_HI32 / GATE_VALUE_LO32: the two halves of a wide (128-bit) integer sum: v = (v >> 32) * 2^32 + (v & 0xffffffff);
 // each half is summed in its own int64 slot (exact for < 2^31 rows per execution), recombined on the host
 // GATE_STRREF: the value is a STRING column held by reference (address of its record; SlotSpec.table = its TABLE_KEYPTR table)
-enum SlotGate { GATE_VALUE = 0, GATE_NONNULL_COUNT = 1, GATE_ONE = 2, GATE_VALUE_HI32 = 3, GATE_VALUE_LO32 = 4, GATE_STRREF = 5 };
+// GATE_LIMB0..3: the four 32-bit limbs of a wide DECIMAL (precision > 18) value v = l3 * 2^96 + l2 * 2^64 + l1 * 2^32 + l0
+// (l0..l2 unsigned, l3 signed); each summed in its own int64 slot (exact for < 2^31 rows per execution), recombined on the host
+// GATE_DECREF: the value is a wide DECIMAL column held by reference (address of its [len][bytes] record)
+enum SlotGate { GATE_VALUE = 0, GATE_NONNULL_COUNT = 1, GATE_ONE = 2, GATE_VALUE_HI32 = 3, GATE_VALUE_LO32 = 4, GATE_STRREF = 5,
+                GATE_LIMB0 = 6, GATE_LIMB1 = 7, GATE_LIMB2 = 8, GATE_LIMB3 = 9, GATE_DECREF = 10 };
 
 struct SlotSpec {
   int op;     // SLOT_*
@@ -45,6 +49,7 @@ struct AggMap {
   int value_slot2;  // DECIMAL SUM/AVG: the low-half slot (value_slot holds the high half); -1 otherwise
   int in_ps;        // DECIMAL input: (precision << 8) | scale; 0 otherwise
   int buf_ps;       // DECIMAL buffer: SUM/AVG (p + 10, s) bounded to 38; MIN/MAX = input
+  int limb_slot[4]; // SUM/AVG of a wide DECIMAL: the slots of limbs 0..3 (value_slot = limb 3, value_slot2 = -1); else -1
 };
 
 // field type codes used for rows on the host: sd_type in the low byte, DECIMAL precision/scale above it
@@ -66,6 +71,7 @@ struct PlanSpec {
   // analysis
   std::vector<int> expr_nullable;
   std::vector<int> kinds;            // K_* per scan column
+  std::vector<char> lit_wide;        // per literal slot: 1 when it holds a wide DECIMAL (value given as bytes)
   std::vector<TableSpec> tables;
   std::vector<SlotSpec> slots;
   std::vector<AggMap> agg_map;
@@ -110,6 +116,11 @@ std::vector<int> final_field_types(const PlanSpec& p);
 bool type_is_integral(int t);
 bool type_is_fp(int t);
 int kind_of_type(int t);
+// a DECIMAL of more than 18 digits: unscaled values do not fit int64 (records by reference in the kernel, __int128 values)
+inline bool wide_decimal(int type, int precision) { return type == SD_DECIMAL && precision > 18; }
+bool node_is_wide(const PlanSpec& p, int node);
+// K_* of a scan column (a wide DECIMAL column travels as the 32-bit position of its record, like a raw STRING)
+int kind_of_column(const sd_column& c);
 
 }  // namespace sd
 #endif

@@ -375,6 +375,9 @@ int compact(sd_store* s, const int32_t* bucket_ids, int32_t nbuckets, double min
       const int type = s->schema[t].type;
       if (!c.unsupported.empty())
         return set_error(SD_ERR_UNSUPPORTED, "sd_store_compact: batch %lld column %d: %s", (long long)b->batch_id, t, c.unsupported.c_str());
+      if (wide_decimal(type, s->schema[t].precision))
+        return set_error(SD_ERR_UNSUPPORTED, "sd_store_compact: batch %lld column %d: a DECIMAL wider than 18 digits is not re-encoded on the device",
+                         (long long)b->batch_id, t);
       if (c.raw_str)
         return set_error(SD_ERR_UNSUPPORTED, "sd_store_compact: batch %lld column %d: an Uncompressed STRING column is not re-encoded on the device",
                          (long long)b->batch_id, t);

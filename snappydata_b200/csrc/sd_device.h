@@ -152,8 +152,10 @@ enum : int32_t { TABLE_PRIVATE = 0, TABLE_SHARED_ATOMIC = 1, TABLE_GLOBAL_ATOMIC
 // SLOT_MIN_STR / SLOT_MAX_STR: the slot holds the device address of the winning value's [len][bytes] record (0: no value yet);
 // values compare as unsigned bytes (MIN / MAX over STRING: the aggregate buffer is not fixed-width, which is what sends the
 // reference down its ObjectHashSet path, SnappyHashAggregateExec.scala:82-94)
+// SLOT_MIN_DEC / SLOT_MAX_DEC: the same for a DECIMAL wider than 18 digits, whose record is [len][big-endian two's-complement
+// unscaled value]; records compare by their numeric value
 enum : int32_t { SLOT_ADD_F64 = 0, SLOT_ADD_I64 = 1, SLOT_MIN_I64 = 2, SLOT_MAX_I64 = 3, SLOT_MIN_F64 = 4, SLOT_MAX_F64 = 5,
-                 SLOT_MIN_STR = 6, SLOT_MAX_STR = 7 };
+                 SLOT_MIN_STR = 6, SLOT_MAX_STR = 7, SLOT_MIN_DEC = 8, SLOT_MAX_DEC = 9 };
 
 struct ScanArgs {
   const void* batches;            // DevBatch<NC>[nbatches]
@@ -176,7 +178,8 @@ struct ScanArgs {
   int64_t out_cap;                // MODE_PROJECT: capacity in records
   int32_t batch_base;             // MODE_PROJECT: ordinal of this launch's first batch within the execution
   int32_t chunk_rows;             // rows per work item (multiple of every tile size; default CHUNK_ROWS)
-  const uint8_t* lit_pool;        // bytes of the STRING literals of this execution (literal slot k: lits.i[k] = offset << 32 | length)
+  const uint8_t* lit_pool;        // bytes of the STRING literals of this execution (literal slot k: lits.i[k] = offset << 32 | length);
+                                  // a wide DECIMAL literal is its 16-byte little-endian unscaled value there, 16-byte aligned
   int32_t fresh;                  // 1: first launch of an execution -- the last CTA OVERWRITES `result` (no host-side
                                   // identity upload, one dependent operation less in front of the kernel)
   int32_t pad2_;

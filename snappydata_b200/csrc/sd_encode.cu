@@ -416,6 +416,10 @@ extern "C" int sd_store_encode_batch(sd_store* s, int32_t num_rows, const sd_raw
     int* d_slots = nullptr; int* d_count = nullptr; int2* d_pairs = nullptr; uint32_t cap = 0;
   };
   std::vector<Work> work;
+  for (int c = 0; c < ncols; c++)   // before anything is copied: the store stays unchanged
+    if (cols[c].values && wide_decimal(s->schema[c].type, s->schema[c].precision))
+      return set_error(SD_ERR_UNSUPPORTED, "column %d: DECIMAL(%d,%d) is wider than 18 digits: the device encoder writes int64 unscaled values only", c,
+                       s->schema[c].precision, s->schema[c].scale);
   // ---- phase 1: raw values to the device; null words; distinct strings -------------------------------------------------
   for (int c = 0; c < ncols; c++) {
     if (!cols[c].values) continue;

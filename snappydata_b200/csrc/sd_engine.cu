@@ -33,9 +33,20 @@ struct HVal {
   int64_t i = 0;
   double d = 0;
   i128 w = 0;      // DECIMAL unscaled value (any precision); `i` mirrors it when the precision is <= 18
+  // merge of wide-DECIMAL SUM / AVG buffers (wide_acc_add): the exact total as acc_hi * 2^64 + acc_lo, and whether an input
+  // had already overflowed
+  unsigned __int128 acc_lo = 0;
+  i128 acc_hi = 0;
+  bool acc = false, ovf = false;
   std::string s;
 };
 i128 pow10_128(int k) { i128 r = 1; for (int j = 0; j < k; j++) r *= 10; return r; }
+// BigInteger(bytes): big-endian two's complement, 1..16 bytes (a wide DECIMAL record's or literal's unscaled value)
+i128 dec_from_bytes(const uint8_t* b, size_t n) {
+  unsigned __int128 u = (unsigned __int128)(i128)(int8_t)b[0];
+  for (size_t k = 1; k < n; k++) u = (u << 8) | b[k];
+  return (i128)u;
+}
 
 int cmp_str(const std::string& a, const std::string& b) {
   size_t n = std::min(a.size(), b.size());
@@ -159,10 +170,16 @@ Tri tri_cmp(const HVal& a, const HVal& b, int t, bool le) {
   const int c = cmp_hval(a, b, t);
   return {false, le ? c <= 0 : c < 0};
 }
-HVal lit_val(const sd_literal& l, int t) {
+HVal lit_val(const sd_literal& l, int t, bool wide_slot = false) {
   HVal v;
   v.isnull = l.is_null != 0;
+  if (wide_slot) {   // a literal slot of a DECIMAL wider than 18 digits: its unscaled value as bytes
+    if (!l.s || l.slen < 1 || l.slen > 16) v.isnull = true;   // (sd_plan_set_literals refuses such a value)
+    else if (!v.isnull) v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(l.s), (size_t)l.slen);
+    return v;
+  }
   v.i = l.i;
+  v.w = l.i;   // DECIMAL (precision <= 18): cmp_hval compares .w
   v.d = t == SD_FLOAT ? (double)(float)l.d : l.d;
   if (l.s && l.slen > 0) v.s.assign(l.s, (size_t)l.slen);
   return v;
@@ -172,6 +189,8 @@ struct StatEval {
   const PlanSpec& p;
   const std::vector<sd_literal>& lits;
   const uint8_t* stats; int64_t slen; int nfields; int num_rows;
+  int node_col(int a, int b) const { return p.exprs[a].op == SD_OP_COL ? a : b; }
+  static bool wide_ft(int ft) { return ft_base(ft) == SD_DECIMAL && ft_precision(ft) > 18; }
   bool stat(int ord, int which, int type, HVal* out) const {   // which: 0 lower, 1 upper, 2 nullCount
     const int idx = 1 + 3 * ord + which;
     return idx < nfields && unsafe_field(stats, slen, nfields, idx, which == 2 ? (int)SD_INT : type, out);
@@ -200,9 +219,10 @@ struct StatEval {
         const sd_expr& ec = cl ? ea : eb;
         const sd_expr& el = cl ? eb : ea;
         const int t = ec.type, ord = p.cols[ec.a].table_ordinal;
+        const int ft = field_type(t, t == SD_DECIMAL ? decimal_ps(p, node_col(e.a, e.b)) : 0);
         HVal lo, hi;
-        if (!stat(ord, 0, t, &lo) || !stat(ord, 1, t, &hi)) return false;
-        const HVal lit = lit_val(lits[el.a], t);
+        if (!stat(ord, 0, wide_ft(ft) ? ft : t, &lo) || !stat(ord, 1, wide_ft(ft) ? ft : t, &hi)) return false;
+        const HVal lit = lit_val(lits[el.a], wide_ft(ft) ? ft : t, p.lit_wide[(size_t)el.a] != 0);
         int op = e.op;
         if (cr) op = op == SD_OP_LT ? SD_OP_GT : op == SD_OP_LE ? SD_OP_GE : op == SD_OP_GT ? SD_OP_LT : op == SD_OP_GE ? SD_OP_LE : op;
         switch (op) {
@@ -217,13 +237,14 @@ struct StatEval {
       case SD_OP_IN: {
         const sd_expr& ea = p.exprs[e.a];
         if (ea.op != SD_OP_COL || e.c > 200 || e.c < 1) return false;
-        const int t = ea.type, ord = p.cols[ea.a].table_ordinal;
+        const int ord = p.cols[ea.a].table_ordinal;
+        const int t = node_is_wide(p, e.a) ? field_type(SD_DECIMAL, decimal_ps(p, e.a)) : ea.type;
         HVal lo, hi, mn, mx;
         if (!stat(ord, 0, t, &lo) || !stat(ord, 1, t, &hi)) return false;
         bool have = false;
         for (int k = 0; k < e.c; k++) {   // Greatest / Least skip nulls
           if (lits[e.b + k].is_null) continue;
-          const HVal v = lit_val(lits[e.b + k], t);
+          const HVal v = lit_val(lits[e.b + k], t, p.lit_wide[(size_t)(e.b + k)] != 0);
           if (!have) { mn = mx = v; have = true; }
           else { if (cmp_hval(v, mn, t) < 0) mn = v; if (cmp_hval(v, mx, t) > 0) mx = v; }
         }
@@ -919,6 +940,13 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
     std::vector<uint8_t> pool;
     p->lit_packed.assign(p->lits.size(), 0);
     for (size_t i = 0; i < p->lits.size(); i++) {
+      if (p->spec.lit_wide[i]) {   // wide DECIMAL: the 128-bit value, little-endian, 16-byte aligned (sd::dec_lit)
+        pool.resize((pool.size() + 15) & ~size_t(15), 0);
+        p->lit_packed[i] = (int64_t)(((uint64_t)pool.size() << 32) | 16u);
+        const i128 v = p->lits[i].is_null ? 0 : dec_from_bytes(reinterpret_cast<const uint8_t*>(p->lits[i].s), (size_t)p->lits[i].slen);
+        pool.insert(pool.end(), reinterpret_cast<const uint8_t*>(&v), reinterpret_cast<const uint8_t*>(&v) + 16);
+        continue;
+      }
       if (p->lits[i].type != SD_STRING) continue;
       p->lit_packed[i] = (int64_t)(((uint64_t)pool.size() << 32) | (uint32_t)p->lits[i].slen);
       pool.insert(pool.end(), p->lits[i].s, p->lits[i].s + p->lits[i].slen);
@@ -938,7 +966,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   }
   args.lit_pool = p->d_litpool;
   for (size_t i = 0; i < p->lits.size(); i++) {
-    args.lits.i[i] = p->lits[i].type == SD_STRING ? p->lit_packed[i] : p->lits[i].i;
+    args.lits.i[i] = p->lits[i].type == SD_STRING || p->spec.lit_wide[i] ? p->lit_packed[i] : p->lits[i].i;
     args.lits.d[i] = p->lits[i].d;
     if (p->lits[i].is_null) args.lits.nullmask |= 1ull << i;
   }
@@ -1062,7 +1090,8 @@ int fetch_agg_strings(sd_plan* p, const uint64_t* slots, size_t ngroups, StrMap&
   const size_t ns = sp.slots.size();
   std::vector<int64_t> ptrs;
   for (auto& m : sp.agg_map) {
-    if (m.buf_type != SD_STRING) continue;
+    const int op = sp.slots[(size_t)m.value_slot].op;
+    if (m.buf_type != SD_STRING && op != SLOT_MIN_DEC && op != SLOT_MAX_DEC) continue;
     for (size_t g = 0; g < ngroups; g++) { const uint64_t a = slots[g * ns + m.value_slot]; if (a && !out.count(a)) { out.emplace(a, std::string()); ptrs.push_back((int64_t)a); } }
   }
   if (ptrs.empty()) return 0;
@@ -1077,6 +1106,52 @@ int fetch_agg_strings(sd_plan* p, const uint64_t* slots, size_t ngroups, StrMap&
   return 0;
 }
 
+// SUM / AVG buffers of a wide DECIMAL: a total of more than min(38, p + 10) digits is carried through partial rows (and every
+// merge of them) as pow10_128(precision), a value no in-range total reaches, so the final result is NULL however the rows
+// were split into partitions -- the rule one execution applies to all its rows
+static bool wide_sum_overflowed(i128 v, int prec) { return v >= pow10_128(prec) || v <= -pow10_128(prec); }
+// merges add partial totals exactly (each in-range one is below 2^127, so 64-bit halves summed in 128 bits cannot wrap);
+// the total is NULL when an input had overflowed or the exact sum of all of them needs more than `prec` digits
+static void wide_acc_add(HVal& b, const HVal& in, int prec) {
+  if (!b.acc) {
+    b.acc = true;
+    b.ovf = wide_sum_overflowed(b.w, prec);
+    b.acc_lo = (uint64_t)b.w;
+    b.acc_hi = b.w >> 64;
+  }
+  b.ovf = b.ovf || wide_sum_overflowed(in.w, prec);
+  b.acc_lo += (uint64_t)in.w;
+  b.acc_hi += in.w >> 64;
+}
+static void wide_acc_finish(HVal& b, int prec) {
+  if (!b.acc) return;
+  const i128 hi = b.acc_hi + (i128)(b.acc_lo >> 64);
+  const uint64_t lo = (uint64_t)b.acc_lo;
+  b.acc = false;
+  if (b.ovf || hi < -((i128)1 << 63) || hi >= ((i128)1 << 63)) b.w = pow10_128(prec);
+  else {
+    b.w = (i128)(((unsigned __int128)hi << 64) | lo);
+    if (wide_sum_overflowed(b.w, prec)) b.w = pow10_128(prec);
+  }
+  b.i = (int64_t)b.w;
+}
+
+// l3 * 2^96 + l2 * 2^64 + l1 * 2^32 + l0 (l0..l2: sums of unsigned 32-bit limbs, l3: sum of the signed top limbs); *fits = false
+// when the total is outside the int128 range
+static i128 limbs_to_i128(uint64_t l0, uint64_t l1, uint64_t l2, int64_t l3, bool* fits) {
+  uint64_t c = l0;
+  const uint64_t d0 = c & 0xffffffffull;
+  c = l1 + (c >> 32);
+  const uint64_t d1 = c & 0xffffffffull;
+  c = l2 + (c >> 32);
+  const uint64_t d2 = c & 0xffffffffull;
+  const i128 top = (i128)l3 + (i128)(c >> 32);
+  *fits = top >= -((i128)1 << 31) && top < ((i128)1 << 31);
+  if (!*fits) return 0;
+  const unsigned __int128 low = ((unsigned __int128)d2 << 64) | ((unsigned __int128)d1 << 32) | d0;
+  return (i128)(((unsigned __int128)top << 96) | low);
+}
+
 // partial-row fields of one group from its slot values (shared by the dense and the hash paths)
 void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, std::vector<HVal>& vals, const StrMap* strs = nullptr) {
   for (auto& m : sp.agg_map) {
@@ -1087,6 +1162,22 @@ void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, std::vector<HVal>
       if ((m.buf_nullable && cnt == 0) || raw == 0 || !strs) v.isnull = true;
       else { auto it = strs->find(raw); if (it == strs->end()) v.isnull = true; else v.s = it->second; }
       vals.push_back(v);
+      continue;
+    }
+    if (sp.slots[(size_t)m.value_slot].op == SLOT_MIN_DEC || sp.slots[(size_t)m.value_slot].op == SLOT_MAX_DEC) {   // wide MIN / MAX: record address
+      const auto it = strs ? strs->find(raw) : StrMap::const_iterator();
+      if ((m.buf_nullable && cnt == 0) || raw == 0 || !strs || it == strs->end() || it->second.empty() || it->second.size() > 16) v.isnull = true;
+      else { v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(it->second.data()), it->second.size()); v.i = (int64_t)v.w; }
+      vals.push_back(v);
+      continue;
+    }
+    if (m.limb_slot[0] >= 0) {   // SUM / AVG of a wide DECIMAL: four 32-bit limbs summed separately (sd_codegen.cpp build_slots)
+      bool fits = false;
+      v.w = limbs_to_i128(sv[m.limb_slot[0]], sv[m.limb_slot[1]], sv[m.limb_slot[2]], (int64_t)sv[m.limb_slot[3]], &fits);
+      if (!fits || wide_sum_overflowed(v.w, m.buf_ps >> 8)) v.w = pow10_128(m.buf_ps >> 8);   // overflowed: sticky (wide_sum_add)
+      v.i = (int64_t)v.w;
+      if (m.fn == SD_AGG_SUM) { if (m.buf_nullable && cnt == 0) v.isnull = true; vals.push_back(v); }
+      else { vals.push_back(v); HVal c; c.i = cnt; vals.push_back(c); }
       continue;
     }
     if (m.value_slot2 >= 0) {   // DECIMAL SUM / AVG: high and low halves summed separately (sd_codegen.cpp build_slots)
@@ -1177,7 +1268,7 @@ int finish_hash(sd_plan* p) {
   // STRING keys are held by reference (address of the [len][bytes] record in a resident buffer): fetch their bytes
   std::vector<std::vector<std::string>> key_strings((size_t)nk);
   for (int k = 0; k < nk && count; k++) {
-    if (sp.exprs[sp.keys[k]].type != SD_STRING) continue;
+    if (sp.exprs[sp.keys[k]].type != SD_STRING && !node_is_wide(sp, sp.keys[k])) continue;
     rc = fetch_string_records(p->stream, d_keys + k, (int64_t)count, nk, key_strings[(size_t)k]);
     if (rc) { cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor); return rc; }
   }
@@ -1199,6 +1290,11 @@ int finish_hash(sd_plan* p) {
       const int64_t code = hk[(size_t)g * nk + k];
       if ((hn[g] >> k) & 1u) v.isnull = true;
       else if (types[k] == SD_STRING) v.s = key_strings[(size_t)k][g];
+      else if (!key_strings[(size_t)k].empty()) {   // wide DECIMAL key held by reference
+        const std::string& b = key_strings[(size_t)k][g];
+        if (b.empty() || b.size() > 16) return set_error(SD_ERR_CUDA, "corrupt DECIMAL key record (%zu bytes)", b.size());
+        v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(b.data()), b.size()); v.i = (int64_t)v.w;
+      }
       else if (type_is_fp(types[k])) memcpy(&v.d, &code, 8);
       else { v.i = code; v.w = code; }
       vals.push_back(v);
@@ -1224,6 +1320,7 @@ static int project_rows_on_device(sd_plan* p, unsigned long long count, bool* do
   std::vector<int> str_cols;
   for (int j = 0; j < np; j++) {
     const sd_expr& e = sp.exprs[sp.proj[j]];
+    if (node_is_wide(sp, sp.proj[j])) return 0;   // wide DECIMAL records: the host writer below
     switch (e.type) {
       case SD_BOOLEAN: kinds[j] = ROW_KIND_BOOL; break;
       case SD_BYTE: kinds[j] = ROW_KIND_1; break;
@@ -1354,10 +1451,12 @@ int finish_project(sd_plan* p) {
   p->metrics[11] = (int64_t)counters[0];
   std::vector<int> types;
   std::vector<int> str_col(np, -1);
+  std::vector<char> wide(np, 0);   // wide DECIMAL column: the record holds the device address of its [len][bytes] record
   for (int j = 0; j < np; j++) {
     const sd_expr& e = sp.exprs[sp.proj[j]];
     types.push_back(field_type(e.type, e.type == SD_DECIMAL ? decimal_ps(sp, sp.proj[j]) : 0));
     if (e.type == SD_STRING) str_col[j] = e.a;
+    wide[j] = node_is_wide(sp, sp.proj[j]);
   }
   lap("records on the host");
   // strings of raw (variable-width) batches are projected by reference: record = position in the batch's body
@@ -1368,6 +1467,7 @@ int finish_project(sd_plan* p) {
     if (bidx >= p->exec_batches.size()) return set_error(SD_ERR_CUDA, "corrupt projection record (batch %u)", bidx);
     const StoredBatch& sb = *p->exec_batches[bidx];
     for (int j = 0; j < np; j++) {
+      if (wide[j] && !((pnull >> j) & 1u)) { raw_ptrs.push_back((int64_t)r[1 + j]); continue; }
       if (str_col[j] < 0 || ((pnull >> j) & 1u)) continue;
       const StoredCol& sc = sb.cols[sb.positional ? str_col[j] : sp.cols[str_col[j]].table_ordinal];
       if (sc.raw_str) raw_ptrs.push_back((int64_t)(uintptr_t)(sc.dev.dict + (uint32_t)r[1 + j]));
@@ -1397,6 +1497,7 @@ int finish_project(sd_plan* p) {
       const StoredBatch& sb = *p->exec_batches[bidx];
       int64_t var = 0;
       for (int j = 0; j < np; j++) {
+        if (wide[j]) { var += 16; if (!((pnull >> j) & 1u)) nr++; continue; }   // 16 bytes reserved even for NULL (emit_unsafe_row)
         if (str_col[j] < 0 || ((pnull >> j) & 1u)) continue;
         const StoredCol& sc = sb.cols[sb.positional ? str_col[j] : sp.cols[str_col[j]].table_ordinal];
         if (sc.raw_str) { var += ((int64_t)raw_strings[nr++].size() + 7) & ~int64_t(7); continue; }
@@ -1420,6 +1521,19 @@ int finish_project(sd_plan* p) {
     int64_t voff = fixed;
     for (int j = 0; j < np; j++) {
       uint8_t* slot = row + bits + 8 * (int64_t)j;
+      if (wide[j]) {   // (offset << 32 | size) + the record's BigInteger bytes in a 16-byte region
+        int64_t ol = voff << 32;
+        if ((pnull >> j) & 1u) row[j >> 3] |= (uint8_t)(1u << (j & 7));
+        else {
+          const std::string& b = raw_strings[next_raw++];
+          if (b.empty() || b.size() > 16) return set_error(SD_ERR_CUDA, "corrupt DECIMAL record (%zu bytes)", b.size());
+          memcpy(row + voff, b.data(), b.size());
+          ol |= (int64_t)b.size();
+        }
+        memcpy(slot, &ol, 8);
+        voff += 16;
+        continue;
+      }
       if ((pnull >> j) & 1u) { row[j >> 3] |= (uint8_t)(1u << (j & 7)); continue; }
       const uint64_t raw = r[1 + j];
       const int t = ft_base(types[j]);
@@ -1534,6 +1648,9 @@ int sd_plan_set_literals(sd_plan* p, const sd_literal* vals, int32_t n) {
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
   if (n != (int)p->lits.size()) return set_error(SD_ERR_INVALID, "sd_plan_set_literals: plan has %zu literal slots, got %d", p->lits.size(), n);
   if (!p->pending.empty()) return set_error(SD_ERR_STATE, "sd_plan_set_literals: batches already submitted for this execution");
+  for (int i = 0; i < n; i++)
+    if (p->spec.lit_wide[(size_t)i] && !vals[i].is_null && (!vals[i].s || vals[i].slen < 1 || vals[i].slen > 16))
+      return set_error(SD_ERR_INVALID, "sd_plan_set_literals: slot %d holds a DECIMAL wider than 18 digits: its value needs 1..16 bytes (BigInteger.toByteArray)", i);
   for (int i = 0; i < n; i++) {
     p->lits[i] = vals[i];
     p->lit_strs[i].assign(vals[i].s ? vals[i].s : "", vals[i].s ? (size_t)std::max(0, vals[i].slen) : 0);
@@ -1678,9 +1795,16 @@ static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
   }
   for (auto& c : p->spec.cols) {
     if (c.table_ordinal < 0 || c.table_ordinal >= (int)s->schema.size()) return set_error(SD_ERR_INVALID, "plan column ordinal %d outside the store schema", c.table_ordinal);
-    if (s->schema[c.table_ordinal].type != c.type || s->schema[c.table_ordinal].nullable != c.nullable)
+    const sd_column& sc = s->schema[c.table_ordinal];
+    if (sc.type != c.type || sc.nullable != c.nullable)
       return set_error(SD_ERR_INVALID, "plan column %d (type %d nullable %d) does not match the store schema (type %d nullable %d)", c.table_ordinal,
-                       c.type, c.nullable, s->schema[c.table_ordinal].type, s->schema[c.table_ordinal].nullable);
+                       c.type, c.nullable, sc.type, sc.nullable);
+    // a DECIMAL of more than 18 digits is resident as record positions + body, a narrower one as int64 values: the kernel
+    // reads the layout the PLAN's precision implies, so both sides must agree on it (and a wide column's scale on its values)
+    if (c.type == SD_DECIMAL && (wide_decimal(c.type, c.precision) != wide_decimal(sc.type, sc.precision) ||
+                                 (wide_decimal(c.type, c.precision) && c.scale != sc.scale)))
+      return set_error(SD_ERR_INVALID, "plan column %d is DECIMAL(%d,%d), the store column DECIMAL(%d,%d): a DECIMAL of more than 18 digits "
+                       "on one side only, or a different scale of one", c.table_ordinal, c.precision, c.scale, sc.precision, sc.scale);
   }
   std::vector<int32_t> buckets(bucket_ids, bucket_ids + (bucket_ids ? nbuckets : 0));
   const std::string lk = literal_key(p);
@@ -2169,6 +2293,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
       if (!f[k].isnull) {
         if (types[k] == SD_STRING) { uint32_t l = (uint32_t)f[k].s.size(); key.append(reinterpret_cast<char*>(&l), 4); key.append(f[k].s); }
         else if (type_is_fp(types[k])) { double d = f[k].d; if (d == 0.0) d = 0.0; if (std::isnan(d)) d = NAN; key.append(reinterpret_cast<char*>(&d), 8); }
+        else if (ft_base(types[k]) == SD_DECIMAL && ft_precision(types[k]) > 18) key.append(reinterpret_cast<const char*>(&f[k].w), 16);
         else key.append(reinterpret_cast<const char*>(&f[k].i), 8);
       }
     }
@@ -2191,13 +2316,15 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
           case SD_AGG_SUM:
             if (!in.isnull) {
               if (m.buf_type == SD_DOUBLE) b.d = (b.isnull ? 0.0 : b.d) + in.d;
+              else if (m.limb_slot[0] >= 0) { if (b.isnull) b.w = in.w; else wide_acc_add(b, in, m.buf_ps >> 8); }
               else if (m.buf_type == SD_DECIMAL) { b.w = (b.isnull ? (i128)0 : b.w) + in.w; b.i = (int64_t)b.w; }
               else b.i = (int64_t)((uint64_t)(b.isnull ? 0 : b.i) + (uint64_t)in.i);
               b.isnull = false;
             }
             k++; break;
           case SD_AGG_AVG:
-            if (m.buf_type == SD_DECIMAL) { b.w += in.w; b.i = (int64_t)b.w; } else b.d += in.d;
+            if (m.limb_slot[0] >= 0) wide_acc_add(b, in, m.buf_ps >> 8);
+            else if (m.buf_type == SD_DECIMAL) { b.w += in.w; b.i = (int64_t)b.w; } else b.d += in.d;
             g->bufs[k + 1].i += f[nk + k + 1].i; k += 2; break;
           default:
             if (!in.isnull) {
@@ -2223,6 +2350,8 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
   const std::vector<int> otypes = evaluate ? final_field_types(sp) : types;
   std::vector<HVal> vals;
   for (auto& g : groups) {
+    for (size_t a = 0, k = 0; a < sp.agg_map.size(); k += sp.agg_map[a].fn == SD_AGG_AVG ? 2 : 1, a++)
+      if (sp.agg_map[a].limb_slot[0] >= 0) wide_acc_finish(g.bufs[k], sp.agg_map[a].buf_ps >> 8);
     vals.assign(g.keys.begin(), g.keys.end());
     if (!evaluate) vals.insert(vals.end(), g.bufs.begin(), g.bufs.end());
     else {
@@ -2232,7 +2361,22 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
           HVal v;
           const int64_t cnt = g.bufs[k + 1].i;
           if (cnt == 0) v.isnull = true;
-          else if (m.buf_type == SD_DECIMAL) {
+          else if (m.limb_slot[0] >= 0) {
+            // the same quotient for a wide input, whose sum * 10^k may not fit 128 bits: q0 = sum / count, then the k more
+            // digits from the remainder (|remainder| * 10^k < 2^63 * 10^4); a q0 of more than precision - k digits cannot fit
+            const int ft = otypes[vals.size()], kk = ft_scale(ft) - (m.in_ps & 0xff), pr = ft_precision(ft);
+            const i128 sum = g.bufs[k].w, den = cnt, q0 = sum / den, r0 = sum % den;
+            // a sum of more than p + 10 digits is NULL: so is the average
+            if (wide_sum_overflowed(sum, m.buf_ps >> 8) || q0 >= pow10_128(pr - kk) || q0 <= -pow10_128(pr - kk)) v.isnull = true;
+            else {
+              const i128 num1 = r0 * pow10_128(kk);
+              i128 q = q0 * pow10_128(kk) + num1 / den, rem = num1 % den;
+              if (rem < 0) rem = -rem;
+              if (2 * rem >= den) q += (sum < 0 ? -1 : 1);
+              if (q >= pow10_128(pr) || q <= -pow10_128(pr)) v.isnull = true;
+              else { v.w = q; v.i = (int64_t)q; }
+            }
+          } else if (m.buf_type == SD_DECIMAL) {
             // Cast(Cast(sum, DECIMAL(p+14,s+4)) / Cast(count, ...), DECIMAL(p+4,s+4)): the quotient at scale s+4, HALF_UP
             const int ft = otypes[vals.size()];
             const i128 num = g.bufs[k].w * pow10_128(ft_scale(ft) - (m.in_ps & 0xff)), den = cnt;
@@ -2344,7 +2488,10 @@ static bool dense_exchange_eligible(const sd_plan* p) {
   const PlanSpec& sp = p->spec;
   if (sp.mode != MODE_NOKEY && sp.mode != MODE_GROUPS) return false;
   if (p->finished_nrows >= 0) return false;   // rows already materialised by an earlier call
-  for (const auto& sl : sp.slots) if (sl.op == SLOT_MIN_STR || sl.op == SLOT_MAX_STR) return false;   // values live in this rank's HBM
+  for (const auto& sl : sp.slots) if (sl.op == SLOT_MIN_STR || sl.op == SLOT_MAX_STR || sl.op == SLOT_MIN_DEC || sl.op == SLOT_MAX_DEC) return false;
+  // limb sums are exact below 2^31 rows of ONE execution: summing them over the ranks could pass 2^64, so wide-DECIMAL sums
+  // take the by-value exchange, whose merge adds recombined 128-bit totals with an overflow check
+  for (const auto& sl : sp.slots) if (sl.gate >= GATE_LIMB0 && sl.gate <= GATE_LIMB3) return false;   // values live in this rank's HBM
   return true;
 }
 

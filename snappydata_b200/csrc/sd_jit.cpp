@@ -124,7 +124,8 @@ int jit_compile(const PlanSpec& spec, int device, KernelEntry& out) {
   if (nr != NVRTC_SUCCESS) return set_error(SD_ERR_CUDA, "nvrtcCreateProgram: %s", d.GetErrorString(nr));
   d.AddNameExpression(prog, name_expr.c_str());
   // -lineinfo adds ~50 % to the compile: only when a profile of a JIT kernel is wanted (SD_JIT_LINEINFO=1)
-  std::vector<std::string> optv = {"--gpu-architecture=sm_90a", "-std=c++17", "--fmad=false", "-default-device"};
+  // -device-int128: 128-bit integers of the wide-DECIMAL helpers in sd_kernels.cuh (nvcc allows them on sm_90a by default)
+  std::vector<std::string> optv = {"--gpu-architecture=sm_90a", "-std=c++17", "--fmad=false", "-default-device", "-device-int128"};
   const char* li = getenv("SD_JIT_LINEINFO");
   if (li && atoi(li) > 0) optv.push_back("-lineinfo");
   if (const char* defs = getenv("SD_JIT_DEFINES")) {   // space-separated -DNAME=VALUE switches (experiments; part of the plan signature)

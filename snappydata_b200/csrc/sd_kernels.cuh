@@ -103,6 +103,29 @@ static __device__ __noinline__ uint64_t str_hash_rec(const uint8_t* rec) {   // 
   return h ^ (uint64_t)n;
 }
 
+// ---- DECIMAL wider than 18 digits: records are [len:int32 LE][unscaled value as BigInteger.toByteArray: big-endian, minimal
+//      two's complement, 1..16 bytes] (enc/Uncompressed.scala:330-345), read into a 128-bit integer.  NVRTC needs
+//      -device-int128 for them (sd_jit.cpp passes it); without it only plans free of wide DECIMALs compile ------------------
+#if !defined(__CUDACC_RTC__) || defined(__CUDACC_RTC_INT128__)
+#define SD_HAVE_I128 1
+typedef __int128 i128;
+static __device__ __noinline__ i128 dec_rec(const uint8_t* rec) {
+  const int n = rec_len(rec);
+  unsigned __int128 u = (unsigned __int128)(i128)(int8_t)rec[4];   // sign extension from the first byte
+  for (int i = 1; i < n; i++) u = (u << 8) | rec[4 + i];
+  return (i128)u;
+}
+// literal slot of a wide DECIMAL: 16 bytes, little-endian, 16-byte aligned in the literal pool
+__device__ __forceinline__ i128 dec_lit(const uint8_t* p) {
+  const uint64_t* w = reinterpret_cast<const uint64_t*>(p);
+  return (i128)(((unsigned __int128)w[1] << 64) | w[0]);
+}
+__host__ __device__ constexpr i128 p10w(int k) { return k <= 0 ? (i128)1 : (i128)10 * p10w(k - 1); }
+constexpr bool HAVE_I128 = true;
+#else
+constexpr bool HAVE_I128 = false;   // a plan with SLOT_MIN_DEC / SLOT_MAX_DEC slots static_asserts on it (sd_codegen.cpp)
+#endif
+
 // ---- slot (accumulator) algebra: every op is a commutative monoid over 8-byte words ------------
 __device__ __forceinline__ uint64_t f2u(double d) { return (uint64_t)__double_as_longlong(d); }
 __device__ __forceinline__ double u2f(uint64_t u) { return __longlong_as_double((long long)u); }
@@ -114,7 +137,7 @@ __host__ __device__ constexpr uint64_t slot_identity(int op) {
        : op == SLOT_MAX_I64 ? 0x8000000000000000ull
        : op == SLOT_MIN_F64 ? 0x7ff8000000000000ull   /* NaN: the greatest element of the order */
        : op == SLOT_MAX_F64 ? 0xfff0000000000000ull   /* -inf */
-       : 0ull;                                         /* SLOT_MIN_STR / SLOT_MAX_STR: no record yet */
+       : 0ull;                                         /* SLOT_MIN_STR / SLOT_MAX_STR / *_DEC: no record yet */
 }
 __device__ __forceinline__ uint64_t slot_combine(int op, uint64_t a, uint64_t b) {
   switch (op) {
@@ -124,8 +147,14 @@ __device__ __forceinline__ uint64_t slot_combine(int op, uint64_t a, uint64_t b)
     case SLOT_MAX_I64: return (int64_t)b > (int64_t)a ? b : a;
     case SLOT_MIN_F64: return f_lt(u2f(b), u2f(a)) ? b : a;
     case SLOT_MAX_F64: return f_gt(u2f(b), u2f(a)) ? b : a;
-    default: {   // SLOT_MIN_STR / SLOT_MAX_STR: addresses of [len][bytes] records, 0 = none
+    default: {   // SLOT_MIN_STR / SLOT_MAX_STR / SLOT_MIN_DEC / SLOT_MAX_DEC: addresses of [len][bytes] records, 0 = none
       if (a == 0ull || b == 0ull || a == b) return a ? a : b;
+#ifdef SD_HAVE_I128
+      if (op == SLOT_MIN_DEC || op == SLOT_MAX_DEC) {
+        const i128 x = dec_rec(reinterpret_cast<const uint8_t*>(b)), y = dec_rec(reinterpret_cast<const uint8_t*>(a));
+        return (op == SLOT_MIN_DEC ? x < y : x > y) ? b : a;
+      }
+#endif
       const int c = str_cmp_recs(reinterpret_cast<const uint8_t*>(b), reinterpret_cast<const uint8_t*>(a));
       return (op == SLOT_MIN_STR ? c < 0 : c > 0) ? b : a;
     }

@@ -300,8 +300,9 @@ static int64_t parse_dictionary(const uint8_t* p, const uint8_t* end, int type, 
 
 // device_fill_total >= 0: `buf` holds only the buffer's prefix (header, null words, dictionary) and a kernel of the caller
 // writes the whole buffer (device_fill_total bytes) at the device address this function reserves (sd_encode.cu)
+// wide: a DECIMAL column of more than 18 digits (variable-width records, laid out like a raw STRING body)
 static int upload_column(sd_store* s, const uint8_t* buf, int64_t len, int type, int nullable, int num_rows, StoredCol& c,
-                         int64_t device_fill_total = -1) {
+                         int64_t device_fill_total = -1, bool wide = false) {
   if (len < 8) return set_error(SD_ERR_INVALID, "column buffer shorter than its 8-byte header");
   const bool device_fill = device_fill_total >= 0;
   if (device_fill) len = device_fill_total;
@@ -336,7 +337,7 @@ static int upload_column(sd_store* s, const uint8_t* buf, int64_t len, int type,
       if (tid < 0 || tid > ENC_BOOLEAN_BITSET || nb < 0 || (nb & 7) || 8 + (int64_t)nb > ulen) return set_error(SD_ERR_INVALID, "corrupt header in LZ4 column buffer");
       int64_t need = 8 + nb;
       // encodings whose layout needs a host walk over every value (run lengths, variable-width strings): decode it all here
-      if (tid == ENC_RUN_LENGTH || (tid == ENC_UNCOMPRESSED && type == SD_STRING)) need = ulen;
+      if (tid == ENC_RUN_LENGTH || (tid == ENC_UNCOMPRESSED && (type == SD_STRING || wide))) need = ulen;
       if (tid == ENC_DICTIONARY || tid == ENC_BIG_DICTIONARY) {
         need += 4;
         if (want >= need) {
@@ -406,6 +407,23 @@ static int upload_column(sd_store* s, const uint8_t* buf, int64_t len, int type,
   std::vector<int32_t> run_ends, run_codes, str_pos;
   switch (type_id) {
     case ENC_UNCOMPRESSED:
+      if (wide) {
+        // DECIMAL(p > 18): back-to-back [len:int32][unscaled value, BigInteger.toByteArray] (enc/Uncompressed.scala:330-345),
+        // walked like a raw STRING body; a value of precision <= 38 takes 1..16 bytes
+        const uint8_t* q = buf + body;
+        str_pos.reserve((size_t)nn);
+        for (int64_t k = 0; k < nn; k++) {
+          if (q + 4 > end) return set_error(SD_ERR_INVALID, "uncompressed DECIMAL column truncated at value %lld", (long long)k);
+          const int32_t l = rd_i32(q);
+          if (l < 1 || l > 16 || q + 4 + l > end)
+            return set_error(SD_ERR_INVALID, "uncompressed DECIMAL column: value %lld has %d bytes (1..16 expected)", (long long)k, l);
+          if (q - (buf + body) > INT32_MAX) return set_error(SD_ERR_UNSUPPORTED, "uncompressed DECIMAL body beyond 2 GB");
+          str_pos.push_back((int32_t)(q - (buf + body)));
+          q += 4 + l;
+        }
+        c.raw_str = true;
+        break;
+      }
       if (type == SD_STRING) {
         // variable width: back-to-back [len:int32][bytes]; the reference reads it with a sequential cursor
         // (enc/Uncompressed.scala:116-161).  One host walk per buffer gives every stored value's record position, which
@@ -533,7 +551,7 @@ static int upload_column(sd_store* s, const uint8_t* buf, int64_t len, int type,
       c.dev.dict = reinterpret_cast<const uint8_t*>(dc);
     }
   }
-  const int kind = kind_of_type(type);
+  const int kind = wide ? K_CODE : kind_of_type(type);
   c.fast = !c.has_nulls && ((kind == K_CODE && (type_id == ENC_DICTIONARY || type_id == ENC_BIG_DICTIONARY || c.raw_str)) ||
                             (kind != K_CODE && type_id == ENC_UNCOMPRESSED));
   // string values by reference (hash-table keys): device address of every dictionary entry's record
@@ -778,11 +796,18 @@ int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals) {
     if (!buf) continue;
     StoredCol& c = sb->cols[t];
     if (c.present) continue;   // same table column projected twice
-    int rc = upload_column(s, buf, b->col_lens[i], s->schema[t].type, s->schema[t].nullable, b->num_rows, c);
+    const bool wide = wide_decimal(s->schema[t].type, s->schema[t].precision);
+    int rc = upload_column(s, buf, b->col_lens[i], s->schema[t].type, s->schema[t].nullable, b->num_rows, c, -1, wide);
     if (rc) return rc;
     for (int depth = 0; depth < 2; depth++) {
       const void* const* arr = depth == 0 ? b->delta0 : b->delta1;
       const int64_t* lens = depth == 0 ? b->delta0_lens : b->delta1_lens;
+      if (arr && arr[i] && wide) {   // kept, like any delta the engine cannot decode: a scan of this column is refused
+        c.unsupported = "update delta on a DECIMAL wider than 18 digits";
+        sb->has_deltas = true;
+        c.fast = false;
+        continue;
+      }
       if (arr && arr[i]) {
         rc = upload_delta(s, reinterpret_cast<const uint8_t*>(arr[i]), lens[i], s->schema[t].type, c, depth);
         if (rc) return rc;
@@ -899,6 +924,9 @@ int sd_host_unregister(void* p) {
 
 int sd_store_create(int device, int32_t ncols, const sd_column* schema, sd_store** out) {
   if (!out || ncols < 0 || (ncols > 0 && !schema)) return sd::set_error(SD_ERR_INVALID, "sd_store_create: bad arguments");
+  for (int32_t c = 0; c < ncols; c++)
+    if (schema[c].type == SD_DECIMAL && (schema[c].precision < 0 || schema[c].precision > 38))
+      return sd::set_error(SD_ERR_INVALID, "sd_store_create: DECIMAL column %d needs precision <= 38 (got %d)", c, schema[c].precision);
   int ndev = 0;
   SD_CUDA(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return sd::set_error(SD_ERR_INVALID, "sd_store_create: device %d of %d", device, ndev);
