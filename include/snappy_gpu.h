@@ -112,9 +112,26 @@ typedef struct sd_expr {
  * Wide DECIMAL input (precision > 18): SUM / AVG sum each value as four 32-bit limbs (exact below 2^31 rows per execution),
  * a total of more than min(38, p+10) digits is NULL -- in partial rows such a total is written as 10^(buffer precision), a
  * value no in-range total reaches, and the merges keep it so (they add partial totals exactly); MIN / MAX keep the input type; AVG's result is
- * DECIMAL(min(38,p+4), min(38,s+4)) rounded HALF_UP, NULL when it does not fit. */
+ * DECIMAL(min(38,p+4), min(38,s+4)) rounded HALF_UP, NULL when it does not fit.
+ * Moment aggregates (Spark 2.1.1 CentralMomentAgg; stddev / variance are the SAMP forms).  The input node must be DOUBLE (Spark
+ * casts any other numeric child to DOUBLE, an SD_OP_CAST node here), else SD_ERR_INVALID.  Buffers are non-nullable DOUBLEs,
+ * 0.0 before any input, in aggBufferAttributes order:
+ *   STDDEV_POP / STDDEV_SAMP / VAR_POP / VAR_SAMP : [n, avg, m2]
+ *   SKEWNESS                                      : [n, avg, m2, m3]
+ *   KURTOSIS                                      : [n, avg, m2, m3, m4]
+ * (m_k = sum (x - avg)^k over the non-null inputs).  Merge is Spark's (Chan et al.):
+ *   n = n1+n2, d = avg2-avg1, dN = n == 0 ? 0 : d/n, avg = avg1 + dN*n2, m2 = m2_1+m2_2 + d*dN*n1*n2,
+ *   m3 = m3_1+m3_2 + dN^2*d*n1*n2*(n1-n2) + 3dN*(n1*m2_2 - n2*m2_1),
+ *   m4 = m4_1+m4_2 + dN^3*d*n1*n2*(n1^2-n1*n2+n2^2) + 6dN^2*(n1^2*m2_2 + n2^2*m2_1) + 4dN*(n1*m3_2 - n2*m3_1).
+ * Results are DOUBLE, NULL when n == 0; VAR_POP m2/n; VAR_SAMP NaN when n == 1, else m2/(n-1); STDDEV_* their square roots;
+ * SKEWNESS NaN when m2 == 0, else sqrt(n)*m3/sqrt(m2^3); KURTOSIS NaN when m2 == 0, else n*m4/m2^2 - 3.  A NaN or +-Inf input
+ * makes the group's results NaN.  The device sums (x - K)^j around one shift K per group and input (the first value the group
+ * sees) and the partial rows carry the buffers above; plans with moment aggregates have no dense partials export
+ * (sd_plan_partials_layout / sd_plan_export_partials / sd_plan_import_partials: SD_ERR_UNSUPPORTED). */
 typedef enum sd_agg_fn {
-  SD_AGG_COUNT_STAR = 1, SD_AGG_COUNT = 2, SD_AGG_SUM = 3, SD_AGG_AVG = 4, SD_AGG_MIN = 5, SD_AGG_MAX = 6
+  SD_AGG_COUNT_STAR = 1, SD_AGG_COUNT = 2, SD_AGG_SUM = 3, SD_AGG_AVG = 4, SD_AGG_MIN = 5, SD_AGG_MAX = 6,
+  SD_AGG_STDDEV_POP = 7, SD_AGG_STDDEV_SAMP = 8, SD_AGG_VAR_POP = 9, SD_AGG_VAR_SAMP = 10, SD_AGG_SKEWNESS = 11,
+  SD_AGG_KURTOSIS = 12
 } sd_agg_fn;
 
 typedef struct sd_agg {
@@ -361,7 +378,8 @@ int sd_plan_execute_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, in
 
 /* ---- export of the dense partial table for an on-device exchange (NCCL all-reduce over NVLink of
  *      per-GPU partials; SURVEY.md 8e).  Writes nslots int64/double words per group into dev_out
- *      (device pointer) on the plan's stream.  Only for plans without string/hash keys. ---------- */
+ *      (device pointer) on the plan's stream.  Only for plans without string/hash keys, and without moment aggregates
+ *      (their shifted sums of different GPUs do not add). ---------------------------------------------------------- */
 int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32_t* slot_is_f64);
 int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes);
 int sd_plan_import_partials(sd_plan* p, const void* dev_in, int64_t bytes);

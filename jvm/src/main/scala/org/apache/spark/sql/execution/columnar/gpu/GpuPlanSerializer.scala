@@ -50,6 +50,9 @@ private[gpu] object Abi {
   final val IN = 35; final val STARTSWITH = 36
   // sd_agg_fn
   final val COUNT_STAR = 1; final val COUNT = 2; final val SUM = 3; final val AVG = 4; final val MIN = 5; final val MAX = 6
+  // CentralMomentAgg: the child is DOUBLE (ImplicitCastInputTypes puts a Cast in front of any other numeric input)
+  final val STDDEV_POP = 7; final val STDDEV_SAMP = 8; final val VAR_POP = 9; final val VAR_SAMP = 10; final val SKEWNESS = 11
+  final val KURTOSIS = 12
   // struct sizes / offsets (x86-64; jvm/abi_offsets.txt is generated from the ctypes mirror and checked by the tests)
   final val SIZEOF_COLUMN = 20; final val SIZEOF_EXPR = 20; final val SIZEOF_AGG = 8; final val SIZEOF_DESC = 104
   final val SIZEOF_LITERAL = 40
@@ -203,6 +206,17 @@ object GpuPlanSerializer {
             case Average(c) => (Abi.AVG, b.add(c))
             case Min(c) => (Abi.MIN, b.add(c))
             case Max(c) => (Abi.MAX, b.add(c))
+            case m @ (StddevPop(_) | StddevSamp(_) | VariancePop(_) | VarianceSamp(_) | Skewness(_) | Kurtosis(_)) =>
+              val c = m.children.head
+              val fn = m match {
+                case _: StddevPop => Abi.STDDEV_POP
+                case _: StddevSamp => Abi.STDDEV_SAMP
+                case _: VariancePop => Abi.VAR_POP
+                case _: VarianceSamp => Abi.VAR_SAMP
+                case _: Skewness => Abi.SKEWNESS
+                case _ => Abi.KURTOSIS
+              }
+              (fn, b.add(c))
             case f => throw new Unsupported(s"aggregate function ${f.prettyName}")
           }
         }.toArray

@@ -48,6 +48,12 @@ class Op:
 
 class AggFn:
     COUNT_STAR, COUNT, SUM, AVG, MIN, MAX = 1, 2, 3, 4, 5, 6
+    # moment aggregates (Spark 2.1.1 CentralMomentAgg) over a DOUBLE input; stddev / variance are the SAMP forms
+    STDDEV_POP, STDDEV_SAMP, VAR_POP, VAR_SAMP, SKEWNESS, KURTOSIS = 7, 8, 9, 10, 11, 12
+
+
+# partial buffers of a moment aggregate, all non-nullable DOUBLE: [n, avg, m2] + [m3] (SKEWNESS) + [m3, m4] (KURTOSIS)
+MOMENT_BUFFERS = {AggFn.STDDEV_POP: 3, AggFn.STDDEV_SAMP: 3, AggFn.VAR_POP: 3, AggFn.VAR_SAMP: 3, AggFn.SKEWNESS: 4, AggFn.KURTOSIS: 5}
 
 
 class sd_column(C.Structure):
@@ -379,6 +385,8 @@ class PlanDesc:
             elif fn == AggFn.AVG:
                 st = self._sum_type(e)
                 out += [st if isinstance(st, tuple) else SqlType.DOUBLE, SqlType.LONG]
+            elif fn in MOMENT_BUFFERS:
+                out += [SqlType.DOUBLE] * MOMENT_BUFFERS[fn]
             else:
                 out.append(self._ftype(e))
         return out
@@ -396,6 +404,8 @@ class PlanDesc:
                     out.append((SqlType.DECIMAL, min(38, p + 4), min(38, s + 4)))
                 else:
                     out.append(SqlType.DOUBLE)
+            elif fn in MOMENT_BUFFERS:
+                out.append(SqlType.DOUBLE)
             else:
                 out.append(self._ftype(e))
         return out

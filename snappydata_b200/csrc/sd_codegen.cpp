@@ -39,7 +39,10 @@ static const char* col_ctype(const sd_column& c);
 std::vector<int> partial_field_types(const PlanSpec& p) {
   std::vector<int> t;
   for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
-  for (auto& m : p.agg_map) { t.push_back(field_type(m.buf_type, m.buf_ps)); if (m.fn == SD_AGG_AVG) t.push_back(SD_LONG); }
+  for (auto& m : p.agg_map) {
+    if (is_moment(m.fn)) { t.insert(t.end(), (size_t)agg_buffer_fields(m.fn), SD_DOUBLE); continue; }
+    t.push_back(field_type(m.buf_type, m.buf_ps)); if (m.fn == SD_AGG_AVG) t.push_back(SD_LONG);
+  }
   return t;
 }
 std::vector<int> final_field_types(const PlanSpec& p) {
@@ -303,12 +306,30 @@ struct Gen {
     for (auto& a : p.aggs) {
       AggMap m;
       memset(&m, 0, sizeof(m));
-      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1;
+      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1; m.shift = -1;
       for (int& l : m.limb_slot) l = -1;
+      for (int& s : m.pow_slot) s = -1;
       const int it = a.expr >= 0 ? p.exprs[a.expr].type : SD_LONG;
       const int in_null = a.expr >= 0 ? static_nullable(a.expr) : 0;
       m.in_type = it;
       if (a.fn != SD_AGG_COUNT_STAR && a.expr < 0) return fail(SD_ERR_INVALID, "aggregate without input expression");
+      if (is_moment(a.fn)) {
+        // n = the non-null count, S_j = sum (x - K)^j around the group's shift K; the host turns them into Spark's buffers
+        if (it != SD_DOUBLE) return fail(SD_ERR_INVALID, "STDDEV / VARIANCE / SKEWNESS / KURTOSIS need a DOUBLE input (cast it)");
+        m.buf_type = SD_DOUBLE;
+        m.value_slot2 = -1;
+        m.count_slot = count_slot_for(a.expr);
+        const int order = moment_order(a.fn);
+        for (int j = 0; j < order; j++) m.pow_slot[j] = add_slot(SLOT_ADD_F64, a.expr, GATE_POW1 + j);
+        m.value_slot = m.pow_slot[0];
+        for (size_t i = 0; i < p.shifts.size(); i++) if (p.shifts[i].pow_slot[0] == m.pow_slot[0]) m.shift = (int)i;   // same input
+        if (m.shift < 0) { p.shifts.push_back(ShiftSpec{0, {-1, -1, -1, -1}}); m.shift = (int)p.shifts.size() - 1; }
+        ShiftSpec* sh = &p.shifts[(size_t)m.shift];
+        for (int j = 0; j < order; j++) sh->pow_slot[j] = m.pow_slot[j];
+        sh->order = std::max(sh->order, order);
+        p.agg_map.push_back(m);
+        continue;
+      }
       if (a.expr >= 0 && it == SD_STRING && a.fn != SD_AGG_COUNT) {
         // MIN / MAX over a STRING column: the slot holds the address of the winning value's record (compared by bytes)
         if (!(a.fn == SD_AGG_MIN || a.fn == SD_AGG_MAX) || p.exprs[a.expr].op != SD_OP_COL)
@@ -710,6 +731,8 @@ struct Gen {
         slt << NL << " ? 0ull : (uint64_t)(uint32_t)((unsigned __int128)" << V << " >> " << 32 * (x.gate - GATE_LIMB0) << ");\n";
       else if (x.gate == GATE_VALUE_HI32) slt << NL << " ? 0ull : (uint64_t)((int64_t)" << V << " >> 32);\n";
       else if (x.gate == GATE_VALUE_LO32) slt << NL << " ? 0ull : ((uint64_t)(int64_t)" << V << " & 0xffffffffull);\n";
+      else if (x.gate == GATE_POW1) slt << NL << " ? sd::SHIFT_EMPTY : sd::shift_cand((double)" << V << ");\n";
+      else if (x.gate >= GATE_POW2 && x.gate <= GATE_POW4) slt << "0ull;\n";
       else {
         const bool f = x.op == SLOT_ADD_F64 || x.op == SLOT_MIN_F64 || x.op == SLOT_MAX_F64;
         char ident[32];
@@ -766,6 +789,17 @@ struct Gen {
     for (int s = 0; s < ns; s++) o << "s == " << s << " ? " << p.slots[s].op << " : ";
     o << "0; }\n";
     o << "  __device__ static __forceinline__ int slot_op_rt(int s) { return slot_op(s); }\n";
+    if (!p.shifts.empty()) {   // moment aggregates (sd_kernels.cuh apply_shifts)
+      const int nsh = (int)p.shifts.size();
+      o << "  static constexpr int NSHIFT = " << nsh << ";\n";
+      o << "  __host__ __device__ static constexpr int order(int i) { return ";
+      for (int i = 0; i < nsh; i++) o << "i == " << i << " ? " << p.shifts[i].order << " : ";
+      o << "0; }\n";
+      o << "  __host__ __device__ static constexpr int pow_slot(int i, int j) { return ";
+      for (int i = 0; i < nsh; i++)
+        for (int j = 1; j <= p.shifts[i].order; j++) o << "(i == " << i << " && j == " << j << ") ? " << p.shifts[i].pow_slot[j - 1] << " : ";
+      o << "0; }\n";
+    }
     o << "  struct Row {\n";
     for (int c = 0; c < nc; c++) o << "    " << col_ctype(p.cols[c]) << " c" << c << "; bool n" << c << ";\n";
     o << "    template <int C, class T> __device__ __forceinline__ void set(T v, bool isnull) {\n";
@@ -865,6 +899,7 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
     if (out.stages == 0) out.reg_groups = 0;   // the register tables are reduced through the ring's memory
   }
   if (!projection) { rc = g.build_slots(); if (rc) return rc; }
+  if (!out.shifts.empty()) out.reg_groups = 0;   // register tables would need a K lookup per row and group: never built for them
   return g.generate();
 }
 

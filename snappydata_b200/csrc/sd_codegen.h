@@ -28,8 +28,11 @@ struct TableSpec {
 // GATE_LIMB0..3: the four 32-bit limbs of a wide DECIMAL (precision > 18) value v = l3 * 2^96 + l2 * 2^64 + l1 * 2^32 + l0
 // (l0..l2 unsigned, l3 signed); each summed in its own int64 slot (exact for < 2^31 rows per execution), recombined on the host
 // GATE_DECREF: the value is a wide DECIMAL column held by reference (address of its [len][bytes] record)
+// GATE_POW1..4: S_j = sum (x - K)^j of a moment aggregate's input (the row leaves its candidate K, x, in S_1;
+// sd_kernels.cuh apply_shifts fills them all once the group's K is known)
 enum SlotGate { GATE_VALUE = 0, GATE_NONNULL_COUNT = 1, GATE_ONE = 2, GATE_VALUE_HI32 = 3, GATE_VALUE_LO32 = 4, GATE_STRREF = 5,
-                GATE_LIMB0 = 6, GATE_LIMB1 = 7, GATE_LIMB2 = 8, GATE_LIMB3 = 9, GATE_DECREF = 10 };
+                GATE_LIMB0 = 6, GATE_LIMB1 = 7, GATE_LIMB2 = 8, GATE_LIMB3 = 9, GATE_DECREF = 10,
+                GATE_POW1 = 11, GATE_POW2 = 12, GATE_POW3 = 13, GATE_POW4 = 14 };
 
 struct SlotSpec {
   int op;     // SLOT_*
@@ -50,6 +53,21 @@ struct AggMap {
   int in_ps;        // DECIMAL input: (precision << 8) | scale; 0 otherwise
   int buf_ps;       // DECIMAL buffer: SUM/AVG (p + 10, s) bounded to 38; MIN/MAX = input
   int limb_slot[4]; // SUM/AVG of a wide DECIMAL: the slots of limbs 0..3 (value_slot = limb 3, value_slot2 = -1); else -1
+  int shift;        // moment aggregate: index of its input's shift in PlanSpec.shifts (count_slot = n, value_slot = S_1); else -1
+  int pow_slot[4];  // moment aggregate: S_1..S_order; else -1
+};
+
+// a moment aggregate (Spark 2.1.1 CentralMomentAgg): STDDEV_* / VAR_* (order 2), SKEWNESS (3), KURTOSIS (4)
+inline bool is_moment(int fn) { return fn >= SD_AGG_STDDEV_POP && fn <= SD_AGG_KURTOSIS; }
+inline int moment_order(int fn) { return fn == SD_AGG_KURTOSIS ? 4 : fn == SD_AGG_SKEWNESS ? 3 : 2; }
+// partial-row buffer fields of an aggregate: AVG [sum, count]; moments [n, avg, m2, (m3, (m4))]; others one
+inline int agg_buffer_fields(int fn) { return fn == SD_AGG_AVG ? 2 : is_moment(fn) ? 1 + moment_order(fn) : 1; }
+
+// one shift K of a plan's moment sums (its K words are not slots, sd_device.h SHIFT_EMPTY): every moment aggregate over the
+// same input shares it and its S_j slots
+struct ShiftSpec {
+  int order;        // highest power summed
+  int pow_slot[4];  // S_1..S_order
 };
 
 // field type codes used for rows on the host: sd_type in the low byte, DECIMAL precision/scale above it
@@ -75,6 +93,7 @@ struct PlanSpec {
   std::vector<TableSpec> tables;
   std::vector<SlotSpec> slots;
   std::vector<AggMap> agg_map;
+  std::vector<ShiftSpec> shifts;     // moment aggregates' shifts: K words [group][shift] beside the slots
   int rows_slot = -1;                // COUNT(*)-like slot that tells which groups exist
   int mode = 0;                      // MODE_NOKEY | MODE_GROUPS | MODE_HASH | MODE_PROJECT | MODE_MUTATE
   int rpt = 4;                       // rows per thread per tile (2, 4, 8)

@@ -134,6 +134,7 @@ struct HashTable {
   int64_t* keys;
   uint32_t* knull;
   uint64_t* vals;
+  uint64_t* shifts;       // [capacity][NSHIFT] K words of moment aggregates (SHIFT_EMPTY when unclaimed), or nullptr
   uint32_t mask;          // capacity - 1 (capacity is a power of two)
   uint32_t max_probe;
   uint32_t* overflow;     // set to 1 when an insert gives up: the host grows the table and replays
@@ -157,6 +158,14 @@ enum : int32_t { TABLE_PRIVATE = 0, TABLE_SHARED_ATOMIC = 1, TABLE_GLOBAL_ATOMIC
 enum : int32_t { SLOT_ADD_F64 = 0, SLOT_ADD_I64 = 1, SLOT_MIN_I64 = 2, SLOT_MAX_I64 = 3, SLOT_MIN_F64 = 4, SLOT_MAX_F64 = 5,
                  SLOT_MIN_STR = 6, SLOT_MAX_STR = 7, SLOT_MIN_DEC = 8, SLOT_MAX_DEC = 9 };
 
+// Moment aggregates (STDDEV / VARIANCE / SKEWNESS / KURTOSIS) sum S_j = sum (x - K)^j around one shift K per group and input.
+// The K words are not slots: they live beside the running result ([ngroups][NSHIFT] after its [ngroups][NSLOT] entries) and
+// beside the hash entries (HashTable.shifts), never in per-thread / per-CTA tables or partials.  A K word is SHIFT_EMPTY until
+// the group's first non-null input claims it with a set-once CAS; every contribution of one execution uses that K, so the sums
+// stay plain commutative additions.  SHIFT_EMPTY is all ones (a byte memset sets it): a NaN no input reaches, because NaN
+// inputs claim the canonical NaN 0x7ff8000000000000.
+constexpr uint64_t SHIFT_EMPTY = 0xffffffffffffffffull;
+
 struct ScanArgs {
   const void* batches;            // DevBatch<NC>[nbatches]
   const int32_t* chunk_prefix;    // [nbatches + 1] cumulative chunk counts
@@ -164,6 +173,7 @@ struct ScanArgs {
   int32_t total_chunks;
   uint64_t* partials;             // [gridDim.x][ngroups * NSLOT] per-CTA partial tables
   uint64_t* result;               // [ngroups * NSLOT] running result (combined into, not overwritten)
+  uint64_t* shifts;               // moment aggregates: [ngroups][NSHIFT] K words (SHIFT_EMPTY until claimed), else nullptr
   unsigned int* ticket;           // CTA completion counter (reset by the last CTA)
   unsigned long long* counters;   // [0] rows scanned, [1] rows that passed the filter
   int32_t ngroups;                // group slots of the dense group table (1 without keys)
@@ -182,7 +192,8 @@ struct ScanArgs {
                                   // a wide DECIMAL literal is its 16-byte little-endian unscaled value there, 16-byte aligned
   int32_t fresh;                  // 1: first launch of an execution -- the last CTA OVERWRITES `result` (no host-side
                                   // identity upload, one dependent operation less in front of the kernel)
-  int32_t pad2_;
+  int32_t shift_cache_off;        // MODE_GROUPS with moment aggregates, TABLE_PRIVATE / TABLE_SHARED_ATOMIC: byte offset in
+                                  // dynamic shared memory of the CTA's copy of the K words, [ngroups][NSHIFT]; -1: none
   Literals lits;
 };
 

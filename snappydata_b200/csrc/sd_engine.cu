@@ -449,12 +449,15 @@ int ensure_result(sd_plan* p, size_t entries) {
   return 0;
 }
 
-// (re)initialise the running result with the slot identities for `ngroups` groups (async: the pinned
+// words of the running result for `ngroups` groups: [ngroups][slots], then the moment aggregates' K words [ngroups][shifts]
+static size_t result_words(const PlanSpec& sp, int ngroups) { return (size_t)ngroups * (sp.slots.size() + sp.shifts.size()); }
+
+// (re)initialise the running result with the slot identities (K words: SHIFT_EMPTY) for `ngroups` groups (async: the pinned
 // staging buffer outlives the copy)
 int init_result(sd_plan* p, int ngroups) {
   const int ns = (int)p->spec.slots.size();
-  const size_t ne = (size_t)ngroups * ns;
-  int rc = ensure_result(p, ne);
+  const size_t ne = (size_t)ngroups * ns, nw = result_words(p->spec, ngroups);
+  int rc = ensure_result(p, nw);
   if (rc) return rc;
   SD_CUDA(cudaStreamSynchronize(p->stream));   // the staging buffer may still be in use by a previous read-back
   uint64_t* hid = p->h_pinned + STATE_HDR;
@@ -463,7 +466,8 @@ int init_result(sd_plan* p, int ngroups) {
     hid[e] = op == SLOT_MIN_I64 ? 0x7fffffffffffffffull : op == SLOT_MAX_I64 ? 0x8000000000000000ull
                    : op == SLOT_MIN_F64 ? 0x7ff8000000000000ull : op == SLOT_MAX_F64 ? 0xfff0000000000000ull : 0ull;
   }
-  SD_CUDA(cudaMemcpyAsync(p->d_result, hid, ne * 8, cudaMemcpyHostToDevice, p->stream));
+  for (size_t e = ne; e < nw; e++) hid[e] = SHIFT_EMPTY;
+  SD_CUDA(cudaMemcpyAsync(p->d_result, hid, nw * 8, cudaMemcpyHostToDevice, p->stream));
   p->result_init = true;
   return 0;
 }
@@ -487,14 +491,14 @@ int key_null(sd_plan* p, int k) {
 
 // when dictionaries grew between launches of one execution the dense group table is re-indexed
 int remap_result(sd_plan* p, const int32_t* old_radix, int old_groups, const int32_t* new_radix, int new_groups) {
-  const int ns = (int)p->spec.slots.size(), nk = (int)p->spec.keys.size();
-  std::vector<uint64_t> oldh((size_t)old_groups * ns);
+  const int ns = (int)p->spec.slots.size(), nk = (int)p->spec.keys.size(), nsh = (int)p->spec.shifts.size();
+  std::vector<uint64_t> oldh(result_words(p->spec, old_groups));
   SD_CUDA(cudaStreamSynchronize(p->stream));
   SD_CUDA(cudaMemcpy(oldh.data(), p->d_result, oldh.size() * 8, cudaMemcpyDeviceToHost));
   int rc = init_result(p, new_groups);
   if (rc) return rc;
   SD_CUDA(cudaStreamSynchronize(p->stream));
-  std::vector<uint64_t> newh((size_t)new_groups * ns);
+  std::vector<uint64_t> newh(result_words(p->spec, new_groups));
   SD_CUDA(cudaMemcpy(newh.data(), p->d_result, newh.size() * 8, cudaMemcpyDeviceToHost));
   for (int g = 0; g < old_groups; g++) {
     int idx[MAX_KEYS], rem = g;
@@ -502,6 +506,7 @@ int remap_result(sd_plan* p, const int32_t* old_radix, int old_groups, const int
     int ng = 0;
     for (int k = 0; k < nk; k++) ng = ng * new_radix[k] + idx[k];
     memcpy(&newh[(size_t)ng * ns], &oldh[(size_t)g * ns], (size_t)ns * 8);
+    if (nsh) memcpy(&newh[(size_t)new_groups * ns + (size_t)ng * nsh], &oldh[(size_t)old_groups * ns + (size_t)g * nsh], (size_t)nsh * 8);
   }
   SD_CUDA(cudaMemcpy(p->d_result, newh.data(), newh.size() * 8, cudaMemcpyHostToDevice));
   return 0;
@@ -653,6 +658,7 @@ void hash_free(sd_plan* p) {
   if (p->hash.keys) cudaFree(p->hash.keys);
   if (p->hash.knull) cudaFree(p->hash.knull);
   if (p->hash.vals) cudaFree(p->hash.vals);
+  if (p->hash.shifts) cudaFree(p->hash.shifts);
   if (p->hash.overflow) cudaFree(p->hash.overflow);
   p->hash = HashTable{};
   p->hash_capacity = 0;
@@ -666,6 +672,7 @@ int hash_ensure(sd_plan* p, uint32_t capacity) {
     SD_CUDA(cudaMalloc(&p->hash.keys, (size_t)capacity * nk * 8));
     SD_CUDA(cudaMalloc(&p->hash.knull, (size_t)capacity * 4));
     SD_CUDA(cudaMalloc(&p->hash.vals, (size_t)capacity * ns * 8));
+    if (!p->spec.shifts.empty()) SD_CUDA(cudaMalloc(&p->hash.shifts, (size_t)capacity * p->spec.shifts.size() * 8));
     SD_CUDA(cudaMalloc(&p->hash.overflow, 1024));   // [0] overflow flag, [8] key count; the rest: diagnostic histograms (SD_EXP_VERIFY builds)
     SD_CUDA(cudaMemset(p->hash.overflow, 0, 1024));
     p->hash.count = p->hash.overflow + 8;
@@ -685,7 +692,7 @@ int hash_ensure(sd_plan* p, uint32_t capacity) {
     SD_CUDA(cudaMemcpy(p->d_hash_ident, id.data(), (size_t)ns * 8, cudaMemcpyHostToDevice));
   }
   if (!p->hash_init) {
-    int rc = hash_table_init(p->stream, p->hash, capacity, ns, p->d_hash_ident);
+    int rc = hash_table_init(p->stream, p->hash, capacity, ns, p->d_hash_ident, (int)p->spec.shifts.size());
     if (rc) return rc;
     p->hash_init = true;
   }
@@ -836,7 +843,8 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   int table_mode = TABLE_PRIVATE;
   int fresh = 0;
   int target_ctas = std::max(1, sp.min_ctas);
-  if (sp.mode == MODE_GROUPS && ngroups <= REG_GROUPS_MAX && k == &p->kernel && p->kernel.staged && getenv("SD_TUNE_REG_GROUPS")) {
+  const int nshift = (int)sp.shifts.size();
+  if (sp.mode == MODE_GROUPS && ngroups <= REG_GROUPS_MAX && k == &p->kernel && p->kernel.staged && getenv("SD_TUNE_REG_GROUPS") && nshift == 0) {
     // experimental (opt-in): measured slower than the private shared-memory tables, see DESIGN.md
     if (p->kernel_reg_state == 0) {
       CodegenOptions opt;
@@ -854,14 +862,18 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   const size_t ring_fixed = 2 * MAX_STAGES * 8 + RING_ALIGN_SLACK;   // mbarriers + alignment of the ring
   const size_t min_ring = k->staged ? ring_fixed + 2 * k->stage_bytes + 128 : 0;
   size_t table_bytes = (size_t)std::max(ns, 1) * (THREADS / 32) * 8;
+  int shift_cache_off = -1;
   if (sp.mode == MODE_GROUPS && table_mode != TABLE_REGS) {
-    const size_t priv = ne * THREADS * 8, shared = ne * 8;
+    // moment aggregates: the shared-memory tables come with the CTA's copy of the K words behind them
+    const size_t kc = (size_t)ngroups * nshift * 8;
+    const size_t priv = ne * THREADS * 8 + kc, shared = ne * 8 + kc;
     // private copies are worth giving up CTAs per SM for; atomics are the last resort
     while (target_ctas > 1 && tile_smem + priv + min_ring > (size_t)p->smem_optin / target_ctas - 1024) target_ctas--;
     const size_t budget1 = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
     if (tile_smem + priv + min_ring <= budget1) { table_mode = TABLE_PRIVATE; table_bytes = priv; }
     else if (shared <= 64 * 1024 && tile_smem + shared + min_ring <= budget1) { table_mode = TABLE_SHARED_ATOMIC; table_bytes = shared; }
     else { table_mode = TABLE_GLOBAL_ATOMIC; table_bytes = 64; }
+    if (nshift > 0 && table_mode != TABLE_GLOBAL_ATOMIC) shift_cache_off = (int)(tile_smem + table_bytes - kc);
   }
   const size_t budget = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
   size_t ring_off = (tile_smem + table_bytes + 127) & ~size_t(127);
@@ -886,8 +898,10 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
       int rc = init_result(p, ngroups);
       if (rc) return rc;
     } else {                                     // the last CTA overwrites it (ScanArgs.fresh): nothing to upload
-      int rc = ensure_result(p, ne);
+      int rc = ensure_result(p, result_words(sp, ngroups));
       if (rc) return rc;
+      // the K words of moment aggregates behind it are claimed, not overwritten: SHIFT_EMPTY (all ones) before the first launch
+      if (nshift) SD_CUDA(cudaMemsetAsync(p->d_result + ne, 0xff, (size_t)ngroups * nshift * 8, p->stream));
       fresh = 1;
       p->result_init = true;
     }
@@ -922,6 +936,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   args.total_chunks = total_chunks;
   args.partials = p->d_partials;
   args.result = p->d_result;
+  args.shifts = nshift ? p->d_result + ne : nullptr;
   args.ticket = p->d_ticket;
   args.counters = p->d_counters;
   args.ngroups = ngroups;
@@ -935,6 +950,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   args.batch_base = batch_base;
   args.chunk_rows = p->chunk_rows;
   args.fresh = fresh;
+  args.shift_cache_off = shift_cache_off;
   memcpy(args.radix, radix, sizeof(radix));
   if (p->litpool_dirty) {   // STRING literal bytes -> device (once per set of literal values)
     std::vector<uint8_t> pool;
@@ -1152,8 +1168,11 @@ static i128 limbs_to_i128(uint64_t l0, uint64_t l1, uint64_t l2, int64_t l3, boo
   return (i128)(((unsigned __int128)top << 96) | low);
 }
 
-// partial-row fields of one group from its slot values (shared by the dense and the hash paths)
-void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, std::vector<HVal>& vals, const StrMap* strs = nullptr) {
+static double u2f_host(uint64_t u) { double d; memcpy(&d, &u, 8); return d; }
+
+// partial-row fields of one group from its slot values and its moment aggregates' K words `kw` (shared by the dense and the
+// hash paths)
+void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, const uint64_t* kw, std::vector<HVal>& vals, const StrMap* strs = nullptr) {
   for (auto& m : sp.agg_map) {
     HVal v;
     const uint64_t raw = sv[m.value_slot];
@@ -1178,6 +1197,23 @@ void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, std::vector<HVal>
       v.i = (int64_t)v.w;
       if (m.fn == SD_AGG_SUM) { if (m.buf_nullable && cnt == 0) v.isnull = true; vals.push_back(v); }
       else { vals.push_back(v); HVal c; c.i = cnt; vals.push_back(c); }
+      continue;
+    }
+    if (is_moment(m.fn)) {   // Spark's buffers [n, avg, m2, (m3, (m4))] from n and S_j = sum (x - K)^j
+      const int order = moment_order(m.fn);
+      double b[5] = {0, 0, 0, 0, 0};
+      if (cnt > 0) {
+        const double n = (double)cnt, K = u2f_host(kw[m.shift]), S1 = u2f_host(sv[m.pow_slot[0]]), S2 = u2f_host(sv[m.pow_slot[1]]);
+        const double S3 = order >= 3 ? u2f_host(sv[m.pow_slot[2]]) : 0.0, S4 = order >= 4 ? u2f_host(sv[m.pow_slot[3]]) : 0.0;
+        const double d = S1 / n;
+        b[0] = n;
+        b[1] = K + d;
+        b[2] = S2 - n * d * d;
+        if (b[2] < 0) b[2] = 0;   // rounding; a NaN stays NaN
+        b[3] = S3 - 3 * d * S2 + 2 * n * d * d * d;
+        b[4] = S4 - 4 * d * S3 + 6 * d * d * S2 - 3 * n * d * d * d * d;
+      }
+      for (int j = 0; j <= order; j++) { HVal f; f.d = b[j]; vals.push_back(f); }
       continue;
     }
     if (m.value_slot2 >= 0) {   // DECIMAL SUM / AVG: high and low halves summed separately (sd_codegen.cpp build_slots)
@@ -1208,7 +1244,7 @@ void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, std::vector<HVal>
 // MODE_HASH: grow + replay on overflow, compact the occupied entries, emit partial rows
 int finish_hash(sd_plan* p) {
   const PlanSpec& sp = p->spec;
-  const int ns = (int)sp.slots.size(), nk = (int)sp.keys.size();
+  const int ns = (int)sp.slots.size(), nk = (int)sp.keys.size(), nsh = (int)sp.shifts.size();
   if (!p->hash_capacity) { int rc = hash_ensure(p, 1u << 16); if (rc) return rc; }
   uint32_t flags[16];
   for (;;) {
@@ -1229,19 +1265,21 @@ int finish_hash(sd_plan* p) {
   }
   const uint32_t count = flags[8];
   // compact -> host
-  int64_t* d_keys = nullptr; uint32_t* d_knull = nullptr; uint64_t* d_vals = nullptr; uint32_t* d_cursor = nullptr;
+  int64_t* d_keys = nullptr; uint32_t* d_knull = nullptr; uint64_t* d_vals = nullptr; uint32_t* d_cursor = nullptr; uint64_t* d_shifts = nullptr;
   const size_t n = std::max<uint32_t>(count, 1);
   SD_CUDA(cudaMalloc(&d_keys, n * std::max(nk, 1) * 8));
   SD_CUDA(cudaMalloc(&d_knull, n * 4));
   SD_CUDA(cudaMalloc(&d_vals, n * ns * 8));
   SD_CUDA(cudaMalloc(&d_cursor, 64));
-  int rc = hash_table_compact(p->stream, p->hash, p->hash_capacity, nk, ns, d_keys, d_knull, d_vals, d_cursor);
+  if (nsh) SD_CUDA(cudaMalloc(&d_shifts, n * nsh * 8));
+  int rc = hash_table_compact(p->stream, p->hash, p->hash_capacity, nk, ns, d_keys, d_knull, d_vals, d_cursor, nsh, d_shifts);
   if (rc) return rc;
   std::vector<int64_t> hk((size_t)count * nk);
   std::vector<uint32_t> hn(count);
-  std::vector<uint64_t> hv((size_t)count * ns);
+  std::vector<uint64_t> hv((size_t)count * ns), hs((size_t)count * nsh);
   unsigned long long counters[2] = {0, 0};
   if (count) {
+    if (nsh) SD_CUDA(cudaMemcpyAsync(hs.data(), d_shifts, hs.size() * 8, cudaMemcpyDeviceToHost, p->stream));
     SD_CUDA(cudaMemcpyAsync(hk.data(), d_keys, hk.size() * 8, cudaMemcpyDeviceToHost, p->stream));
     SD_CUDA(cudaMemcpyAsync(hn.data(), d_knull, hn.size() * 4, cudaMemcpyDeviceToHost, p->stream));
     SD_CUDA(cudaMemcpyAsync(hv.data(), d_vals, hv.size() * 8, cudaMemcpyDeviceToHost, p->stream));
@@ -1270,9 +1308,9 @@ int finish_hash(sd_plan* p) {
   for (int k = 0; k < nk && count; k++) {
     if (sp.exprs[sp.keys[k]].type != SD_STRING && !node_is_wide(sp, sp.keys[k])) continue;
     rc = fetch_string_records(p->stream, d_keys + k, (int64_t)count, nk, key_strings[(size_t)k]);
-    if (rc) { cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor); return rc; }
+    if (rc) { cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor); if (d_shifts) cudaFree(d_shifts); return rc; }
   }
-  cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor);
+  cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor); if (d_shifts) cudaFree(d_shifts);
   update_agg_time(p);
   p->metrics[6] = (int64_t)(p->agg_ms * 1e6);
   p->metrics[8] = (int64_t)counters[0];
@@ -1299,7 +1337,7 @@ int finish_hash(sd_plan* p) {
       else { v.i = code; v.w = code; }
       vals.push_back(v);
     }
-    append_agg_fields(sp, &hv[(size_t)g * ns], vals, &agg_strs);
+    append_agg_fields(sp, &hv[(size_t)g * ns], nsh ? &hs[(size_t)g * nsh] : nullptr, vals, &agg_strs);
     emit_unsafe_row(out, types, vals);
   }
   p->finished_nrows = count;
@@ -1923,12 +1961,12 @@ static int scan_store(sd_plan* p, sd_store* s, const int32_t* bucket_ids, int32_
   return 0;
 }
 
-// dense / no-key state (the [ngroups][slots] table the kernel leaves) -> partial rows appended to `out`:
+// dense / no-key state (the [ngroups][slots] table the kernel leaves, then the K words [ngroups][shifts]) -> partial rows appended to `out`:
 // UnsafeRow(group keys ++ aggregate buffers) (SnappyHashAggregateExec.scala:1148-1178).  The key dictionaries are arguments
 // because the exchange's dense form carries ANOTHER rank's state and dictionaries (ids are private to a partition).
 static int64_t dense_rows_from_state(const PlanSpec& sp, const uint64_t* h, int ngroups, const int32_t* radix, const std::vector<int>& key_null_id,
                                      const std::vector<std::vector<std::string>>& key_vals, const StrMap* agg_strs, std::vector<uint8_t>& out) {
-  const int ns = (int)sp.slots.size(), nk = (int)sp.keys.size();
+  const int ns = (int)sp.slots.size(), nk = (int)sp.keys.size(), nsh = (int)sp.shifts.size();
   const std::vector<int> types = partial_field_types(sp);
   int64_t nrows = 0;
   std::vector<HVal> vals;
@@ -1943,7 +1981,7 @@ static int64_t dense_rows_from_state(const PlanSpec& sp, const uint64_t* h, int 
       if (idx[k] == key_null_id[k]) v.isnull = true; else v.s = key_vals[k][idx[k]];
       vals.push_back(v);
     }
-    append_agg_fields(sp, sv, vals, agg_strs);
+    append_agg_fields(sp, sv, nsh ? h + (size_t)ngroups * ns + (size_t)g * nsh : nullptr, vals, agg_strs);
     emit_unsafe_row(out, types, vals);
     nrows++;
   }
@@ -1957,9 +1995,9 @@ static int finish_dense(sd_plan* p) {
   int rc = 0;
   if (!p->result_init) { rc = init_result(p, 1); if (rc) return rc; p->ngroups = 1; }
   const size_t ne = (size_t)p->ngroups * ns;
-  rc = ensure_result(p, ne);
+  rc = ensure_result(p, result_words(sp, p->ngroups));
   if (rc) return rc;
-  SD_CUDA(cudaMemcpyAsync(p->h_pinned, p->d_state, (STATE_HDR + ne) * 8, cudaMemcpyDeviceToHost, p->stream));   // counters + table in one copy
+  SD_CUDA(cudaMemcpyAsync(p->h_pinned, p->d_state, (STATE_HDR + result_words(sp, p->ngroups)) * 8, cudaMemcpyDeviceToHost, p->stream));   // counters + table in one copy
   SD_CUDA(cudaStreamSynchronize(p->stream));
   const uint64_t* h = p->h_pinned + STATE_HDR;
   const unsigned long long counters[2] = {p->h_pinned[0], p->h_pinned[1]};
@@ -2104,6 +2142,7 @@ void sd_plan_destroy(sd_plan* p) {
 int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32_t* slot_is_f64) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_partials_layout: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
+  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: moment sums of different GPUs are shifted differently and do not add");
   const int ns = (int)p->spec.slots.size();
   if (ngroups) *ngroups = p->ngroups;
   if (nslots) *nslots = ns;
@@ -2114,6 +2153,7 @@ int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_export_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_out) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
+  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: moment sums of different GPUs are shifted differently and do not add");
   SD_CUDA(cudaSetDevice(p->device));
   int rc = flush_pending(p);
   if (rc) return rc;
@@ -2127,6 +2167,7 @@ int sd_plan_import_partials(sd_plan* p, const void* dev_in, int64_t bytes) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_import_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_in) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
+  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: moment sums of different GPUs are shifted differently and do not add");
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
   SD_CUDA(cudaSetDevice(p->device));
@@ -2259,6 +2300,36 @@ int sd_plan_partial_merge(sd_plan* p, const void* partial_rows, int64_t len, voi
   return merge_to_caller(p->spec, partial_rows, len, false, out_rows, cap, out_len, out_nrows);
 }
 
+// CentralMomentAgg (Spark 2.1.1) on the buffers b[0..order] = [n, avg, m2, (m3, (m4))]: mergeExpressions ...
+static void moment_merge(HVal* b, const HVal* in, int order) {
+  const double n1 = b[0].d, n2 = in[0].d, n = n1 + n2;
+  const double delta = in[1].d - b[1].d, dN = n == 0.0 ? 0.0 : delta / n;
+  const double m2a = b[2].d, m2b = in[2].d;
+  const double m3a = order >= 3 ? b[3].d : 0.0, m3b = order >= 3 ? in[3].d : 0.0;
+  b[0].d = n;
+  b[1].d = b[1].d + dN * n2;
+  b[2].d = m2a + m2b + delta * dN * n1 * n2;
+  if (order >= 3) b[3].d = m3a + m3b + dN * dN * delta * n1 * n2 * (n1 - n2) + 3.0 * dN * (n1 * m2b - n2 * m2a);
+  if (order >= 4)
+    b[4].d = b[4].d + in[4].d + dN * dN * dN * delta * n1 * n2 * (n1 * n1 - n1 * n2 + n2 * n2) + 6.0 * dN * dN * (n1 * n1 * m2b + n2 * n2 * m2a) +
+             4.0 * dN * (n1 * m3b - n2 * m3a);
+}
+// ... and evaluateExpression: NULL without input; stddev / variance are the SAMP forms
+static HVal moment_result(int fn, const HVal* b) {
+  HVal v;
+  const double n = b[0].d, m2 = b[2].d;
+  if (n == 0.0) { v.isnull = true; return v; }
+  switch (fn) {
+    case SD_AGG_VAR_POP: v.d = m2 / n; break;
+    case SD_AGG_STDDEV_POP: v.d = std::sqrt(m2 / n); break;
+    case SD_AGG_VAR_SAMP: v.d = n == 1.0 ? NAN : m2 / (n - 1.0); break;
+    case SD_AGG_STDDEV_SAMP: v.d = n == 1.0 ? NAN : std::sqrt(m2 / (n - 1.0)); break;
+    case SD_AGG_SKEWNESS: v.d = m2 == 0.0 ? NAN : std::sqrt(n) * b[3].d / std::sqrt(m2 * m2 * m2); break;
+    default: v.d = m2 == 0.0 ? NAN : n * b[4].d / (m2 * m2) - 3.0; break;   // SD_AGG_KURTOSIS
+  }
+  return v;
+}
+
 static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t len, bool evaluate, std::vector<uint8_t>& out, int64_t* out_nrows) {
   out.clear();
   if (sp.mode == MODE_PROJECT) {   // projected rows of several partitions: concatenation
@@ -2311,6 +2382,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
       for (auto& m : sp.agg_map) {   // mergeExpressions of each function
         HVal& b = g->bufs[k];
         const HVal& in = f[nk + k];
+        if (is_moment(m.fn)) { moment_merge(&b, &in, moment_order(m.fn)); k += agg_buffer_fields(m.fn); continue; }
         switch (m.fn) {
           case SD_AGG_COUNT_STAR: case SD_AGG_COUNT: b.i += in.i; k++; break;
           case SD_AGG_SUM:
@@ -2343,20 +2415,21 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
       HVal v;
       if (m.fn == SD_AGG_SUM || m.fn == SD_AGG_MIN || m.fn == SD_AGG_MAX) v.isnull = true;
       g.bufs.push_back(v);
-      if (m.fn == SD_AGG_AVG) g.bufs.push_back(HVal());
+      for (int j = 1; j < agg_buffer_fields(m.fn); j++) g.bufs.push_back(HVal());   // AVG's count, the moments' 0.0s
     }
     groups.push_back(g);
   }
   const std::vector<int> otypes = evaluate ? final_field_types(sp) : types;
   std::vector<HVal> vals;
   for (auto& g : groups) {
-    for (size_t a = 0, k = 0; a < sp.agg_map.size(); k += sp.agg_map[a].fn == SD_AGG_AVG ? 2 : 1, a++)
+    for (size_t a = 0, k = 0; a < sp.agg_map.size(); k += agg_buffer_fields(sp.agg_map[a].fn), a++)
       if (sp.agg_map[a].limb_slot[0] >= 0) wide_acc_finish(g.bufs[k], sp.agg_map[a].buf_ps >> 8);
     vals.assign(g.keys.begin(), g.keys.end());
     if (!evaluate) vals.insert(vals.end(), g.bufs.begin(), g.bufs.end());
     else {
       int k = 0;
       for (auto& m : sp.agg_map) {
+        if (is_moment(m.fn)) { vals.push_back(moment_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
         if (m.fn == SD_AGG_AVG) {   // Average.evaluateExpression: sum / count, NULL when count == 0
           HVal v;
           const int64_t cnt = g.bufs[k + 1].i;
@@ -2513,7 +2586,7 @@ int sd_plan_exchange(sd_plan* p, sd_comm* c) {
     const size_t ne = (size_t)p->ngroups * ns;
     rc = ensure_result(p, ne);
     if (rc) return rc;
-    state_bytes = (STATE_HDR + ne) * 8;
+    state_bytes = (STATE_HDR + result_words(sp, p->ngroups)) * 8;   // moment aggregates: this rank's K words travel with it
     auto put32 = [&](uint32_t v) { const uint8_t* q = reinterpret_cast<const uint8_t*>(&v); dense_hdr.insert(dense_hdr.end(), q, q + 4); };
     put32((uint32_t)p->ngroups); put32((uint32_t)nk);
     for (int k = 0; k < nk; k++) put32((uint32_t)p->radix[k]);
@@ -2604,8 +2677,8 @@ int sd_plan_exchange(sd_plan* p, sd_comm* c) {
       if ((size_t)radix[k] > vals[(size_t)k].size()) vals[(size_t)k].resize((size_t)radix[k]);
     }
     q = h + 16 + (((size_t)(q - (h + 16)) + 7) & ~size_t(7));
-    if (q + (STATE_HDR + (size_t)ng * ns) * 8 != end) return bad();
-    std::vector<uint64_t> st((STATE_HDR + (size_t)ng * ns));
+    if (q + (STATE_HDR + result_words(sp, (int)ng)) * 8 != end) return bad();
+    std::vector<uint64_t> st(STATE_HDR + result_words(sp, (int)ng));
     memcpy(st.data(), q, st.size() * 8);
     const int64_t nr = dense_rows_from_state(sp, st.data() + STATE_HDR, (int)ng, radix, null_id, vals, nullptr, all);
     if (r == c->rank) {   // this rank's own execution metrics come back with its blob

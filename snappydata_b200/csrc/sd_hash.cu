@@ -14,28 +14,31 @@ __global__ void hash_init_kernel(uint32_t* state, uint64_t* vals, uint32_t capac
 
 __global__ void hash_compact_kernel(const uint32_t* state, const int64_t* keys, const uint32_t* knull, const uint64_t* vals,
                                     uint32_t capacity, int nk, int nslot, int64_t* out_keys, uint32_t* out_knull, uint64_t* out_vals,
-                                    uint32_t* cursor) {
+                                    uint32_t* cursor, const uint64_t* shifts, int nshift, uint64_t* out_shifts) {
   for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < capacity; e += gridDim.x * blockDim.x) {
     if (state[e] != 2u) continue;
     const uint32_t o = atomicAdd(cursor, 1u);
     for (int k = 0; k < nk; k++) out_keys[(size_t)o * nk + k] = keys[(size_t)e * nk + k];
     out_knull[o] = knull[e];
     for (int s = 0; s < nslot; s++) out_vals[(size_t)o * nslot + s] = vals[(size_t)e * nslot + s];
+    for (int s = 0; s < nshift; s++) out_shifts[(size_t)o * nshift + s] = shifts[(size_t)e * nshift + s];
   }
 }
 
-int hash_table_init(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nslot, const uint64_t* d_ident) {
+int hash_table_init(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nslot, const uint64_t* d_ident, int nshift) {
   hash_init_kernel<<<296, 256, 0, stream>>>(t.state, t.vals, capacity, nslot, d_ident);
   SD_CUDA(cudaGetLastError());
+  if (nshift > 0) SD_CUDA(cudaMemsetAsync(t.shifts, 0xff, (size_t)capacity * nshift * 8, stream));   // SHIFT_EMPTY
   SD_CUDA(cudaMemsetAsync(t.overflow, 0, 4, stream));
   SD_CUDA(cudaMemsetAsync(t.count, 0, 4, stream));
   return 0;
 }
 
 int hash_table_compact(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nk, int nslot, int64_t* out_keys,
-                       uint32_t* out_knull, uint64_t* out_vals, uint32_t* d_cursor) {
+                       uint32_t* out_knull, uint64_t* out_vals, uint32_t* d_cursor, int nshift, uint64_t* out_shifts) {
   SD_CUDA(cudaMemsetAsync(d_cursor, 0, 4, stream));
-  hash_compact_kernel<<<296, 256, 0, stream>>>(t.state, t.keys, t.knull, t.vals, capacity, nk, nslot, out_keys, out_knull, out_vals, d_cursor);
+  hash_compact_kernel<<<296, 256, 0, stream>>>(t.state, t.keys, t.knull, t.vals, capacity, nk, nslot, out_keys, out_knull, out_vals, d_cursor,
+                                               t.shifts, nshift, out_shifts);
   SD_CUDA(cudaGetLastError());
   return 0;
 }

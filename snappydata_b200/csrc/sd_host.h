@@ -56,9 +56,10 @@ int kernel_launch(const KernelEntry& k, int grid, size_t smem, cudaStream_t stre
 int jit_compile(const PlanSpec& spec, int device, KernelEntry& out);
 
 // ---- MODE_HASH group table housekeeping (sd_hash.cu) ------------------------------------------------
-int hash_table_init(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nslot, const uint64_t* d_ident);
+// nshift: K words per entry of moment aggregates (t.shifts; sd_device.h SHIFT_EMPTY), copied out to out_shifts by the compaction
+int hash_table_init(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nslot, const uint64_t* d_ident, int nshift);
 int hash_table_compact(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nk, int nslot, int64_t* out_keys,
-                       uint32_t* out_knull, uint64_t* out_vals, uint32_t* d_cursor);
+                       uint32_t* out_knull, uint64_t* out_vals, uint32_t* d_cursor, int nshift, uint64_t* out_shifts);
 // strings held by reference -> host: d_recs[i * stride] = device address of a [len:int32][bytes] record (0: none)
 int fetch_string_records(cudaStream_t stream, const int64_t* d_recs, int64_t n, int64_t stride, std::vector<std::string>& out);
 

@@ -232,6 +232,42 @@ __device__ __forceinline__ int64_t hash_find_or_insert(const HashTable& t, const
   return -1;
 }
 
+// ---- moment aggregates: sums S_j = sum (x - K)^j around one shift K per group ---------------------------------------------
+// A plan with STDDEV / VARIANCE / SKEWNESS / KURTOSIS declares NSHIFT > 0 and, per shift i, order(i) and pow_slot(i, j) for
+// j = 1..order(i).  Its slots() leaves the row's candidate K in the S_1 slot (shift_cand(x), or SHIFT_EMPTY when x is NULL);
+// apply_shifts turns it into the row's contributions once the group's K (sd_device.h SHIFT_EMPTY) is known.  K is a value of the group, so the host's conversion to central moments loses digits to
+// ((mean - K) / sigma)^order, not to (mean / sigma)^order as raw power sums would.
+template <class P, class = void> struct PlanShifts { static constexpr int N = 0; };
+template <class P> struct PlanShifts<P, decltype((void)P::NSHIFT)> { static constexpr int N = P::NSHIFT; };
+
+__device__ __forceinline__ uint64_t shift_cand(double x) { return x != x ? 0x7ff8000000000000ull : f2u(x); }
+// the group's K in the word at p (beside the running result or the hash entry), claimed with `cand` while still SHIFT_EMPTY
+__device__ __forceinline__ uint64_t shift_claim(uint64_t* p, uint64_t cand) {
+  uint64_t k;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(k) : "l"(p) : "memory");
+  if (k == SHIFT_EMPTY) {
+    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(p), SHIFT_EMPTY, cand);
+    k = old == SHIFT_EMPTY ? cand : (uint64_t)old;
+  }
+  return k;
+}
+// kof(i, cand) -> the group's K of shift i
+template <class PLAN, class KOf>
+__device__ __forceinline__ void apply_shifts(uint64_t* sv, KOf&& kof) {
+#pragma unroll
+  for (int i = 0; i < PLAN::NSHIFT; i++) {
+    const uint64_t cand = sv[PLAN::pow_slot(i, 1)];
+    if (cand == SHIFT_EMPTY) { sv[PLAN::pow_slot(i, 1)] = 0ull; continue; }   // NULL input: its sums stay 0
+    const double d = u2f(cand) - u2f(kof(i, cand));
+    double pw = d;
+#pragma unroll
+    for (int j = 1; j <= 4; j++) {
+      if (j <= PLAN::order(i)) sv[PLAN::pow_slot(i, j)] = f2u(pw);
+      pw *= d;
+    }
+  }
+}
+
 // ---- loads ------------------------------------------------------------------------------------
 template <class T> __device__ __forceinline__ T ld_at(const uint8_t* base, int64_t k) {
   return *reinterpret_cast<const T*>(base + k * (int64_t)sizeof(T));
@@ -1102,6 +1138,23 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     for (int e = tid; e < NE; e += THREADS) table[e] = slot_identity(PLAN::slot_op_rt(e % NSLOT));
     consumer_sync();
   }
+  // moment aggregates: where a row finds its group's K (sd_device.h SHIFT_EMPTY).  The words beside the running result / hash
+  // entries hold it; no-key plans keep it in registers once read, private / shared-atomic dense tables a per-CTA copy in shared
+  // memory they fill on first touch
+  constexpr int NSH = PlanShifts<PLAN>::N;
+  static_assert(NSH == 0 || RG == 0, "the register-table variant is never built for plans with moment aggregates");
+  uint64_t kreg[NSH > 0 ? NSH : 1];
+  uint64_t* kcache = nullptr;
+  (void)kreg; (void)kcache;
+  if constexpr (NSH > 0) {
+#pragma unroll
+    for (int i = 0; i < NSH; i++) kreg[i] = SHIFT_EMPTY;
+    if (PLAN::MODE == MODE_GROUPS && args.shift_cache_off >= 0) {
+      kcache = reinterpret_cast<uint64_t*>(smem_raw + args.shift_cache_off);
+      for (int e = tid; e < args.ngroups * NSH; e += THREADS) kcache[e] = SHIFT_EMPTY;
+      consumer_sync();
+    }
+  }
   unsigned long long n_scanned = 0, n_passed = 0;   // flushed from 32-bit per-chunk counters
 
   RowCtx ctx;
@@ -1245,6 +1298,11 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
         uint64_t sv[NSLOT > 0 ? NSLOT : 1];
         PLAN::slots(row, ctx, sv);
         if (PLAN::MODE == MODE_NOKEY) {
+          if constexpr (NSH > 0)
+            apply_shifts<PLAN>(sv, [&](int i, uint64_t c) {
+              if (kreg[i] == SHIFT_EMPTY) kreg[i] = shift_claim(args.shifts + i, c);
+              return kreg[i];
+            });
 #pragma unroll
           for (int s = 0; s < NSLOT; s++) acc[s] = slot_combine(PLAN::slot_op(s), acc[s], sv[s]);
         } else {
@@ -1255,12 +1313,24 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
             const int64_t e = hash_find_or_insert<(PLAN::NKEYS > 0 ? PLAN::NKEYS : 1), PLAN::STRKEYMASK>(args.hash, kc, knull);
             if (e >= 0) {
               uint64_t* t = args.hash.vals + (size_t)e * NSLOT;
+              if constexpr (NSH > 0) apply_shifts<PLAN>(sv, [&](int i, uint64_t c) { return shift_claim(args.hash.shifts + (size_t)e * NSH + i, c); });
 #pragma unroll
               for (int s = 0; s < NSLOT; s++) slot_atomic(PLAN::slot_op(s), t + s, sv[s]);
             }
             continue;
           }
           const int g = PLAN::group(row, ctx);
+          if constexpr (NSH > 0) {
+            uint64_t* kg = args.shifts + (size_t)g * NSH;
+            if (kcache)
+              apply_shifts<PLAN>(sv, [&](int i, uint64_t c) {
+                uint64_t k = kcache[g * NSH + i];
+                if (k == SHIFT_EMPTY) { k = shift_claim(kg + i, c); kcache[g * NSH + i] = k; }
+                return k;
+              });
+            else
+              apply_shifts<PLAN>(sv, [&](int i, uint64_t c) { return shift_claim(kg + i, c); });
+          }
           if (RG > 0) {   // predicated register accumulators: no memory traffic, no dependent smem chains
 #pragma unroll
             for (int gi = 0; gi < RG; gi++) {

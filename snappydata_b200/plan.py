@@ -101,6 +101,14 @@ class PlanBuilder:
     def min(self, e: E): return self.agg(AggFn.MIN, e)
     def max(self, e: E): return self.agg(AggFn.MAX, e)
     def count(self, e: Optional[E] = None): return self.agg(AggFn.COUNT if e is not None else AggFn.COUNT_STAR, e)
+    # moment aggregates take a DOUBLE input, as Spark casts it (ImplicitCastInputTypes): e.cast(SqlType.DOUBLE)
+    def stddev_pop(self, e: E): return self.agg(AggFn.STDDEV_POP, e)
+    def stddev_samp(self, e: E): return self.agg(AggFn.STDDEV_SAMP, e)
+    def var_pop(self, e: E): return self.agg(AggFn.VAR_POP, e)
+    def var_samp(self, e: E): return self.agg(AggFn.VAR_SAMP, e)
+    def skewness(self, e: E): return self.agg(AggFn.SKEWNESS, e)
+    def kurtosis(self, e: E): return self.agg(AggFn.KURTOSIS, e)
+    stddev, variance = stddev_samp, var_samp
     def project(self, *es: E): self._proj = list(es); return self
 
     # UPDATE / DELETE over a resident store (SD_PLAN_MUTATE; the WHERE clause is filter())
