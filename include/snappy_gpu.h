@@ -423,6 +423,15 @@ int sdx_store_batch_info(sd_store* s, int64_t batch_index, int32_t* num_rows, in
  * store asks for generic compression where the device reports support; the hardware then compresses those slabs between
  * L2 and DRAM, invisibly to kernels and copies).  Read only. */
 int sdx_store_memory_info(sd_store* s, int64_t* compressible_bytes, int64_t* slab_bytes);
+/* scan images of a store's current batch versions (narrow byte-aligned copies of NOT NULL columns that the scan kernel's
+ * staged loads read instead of the verbatim values; built and verified on the device when a version is created):
+ * out[0] arena bytes they take, out[1] (batch, column) images, out[2] images whose device verification failed since the
+ * store was created (those columns keep the verbatim path), out[3] microseconds spent building images.  Read only. */
+int sdx_store_image_info(sd_store* s, int64_t out[4]);
+/* the image rule for one column of one batch (host only, no CUDA call): width in bytes (0: no image) of a dictionary image
+ * (dict != 0: DOUBLE / FLOAT with `ndistinct` distinct bit patterns) or of a frame of reference over [lo, hi] (integral
+ * values of elem_bytes 2, 4 or 8 bytes) */
+int sdx_image_width(int32_t dict, int32_t elem_bytes, uint64_t ndistinct, int64_t lo, int64_t hi, int32_t* width);
 /* the batch-skipping decision (ColumnTableScan.scala:820-963) of a plan's filter for one stats row: *pass = 0 when the
  * batch would be skipped.  Host only, no CUDA call (test hook: tests/test_stats_predicate.py compares it with the oracle). */
 int sdx_stats_pass(const sd_plan_desc* desc, const sd_literal* lits, int32_t nlits, const void* stats,
@@ -434,7 +443,9 @@ int sdx_stats_pass(const sd_plan_desc* desc, const sd_literal* lits, int32_t nli
  *   with NULL literal flags ran   [3] stages of the shared-memory ring (0: direct loads)   [4] rows per tile
  *   [5] rows per work item   [6] grid (CTAs)   [7] groups of the dense table (1 without one)   [8..11] batches of the launch
  *   on the BATCH_ALL_FAST, BATCH_FAST_NULLS, BATCH_FAST_OVERLAY and general per-row paths   [12] SDX_REPLAY_*: why the launch
- *   repeats an earlier one of the execution   [13] batches   [14] work items   [15] 0
+ *   repeats an earlier one of the execution   [13] batches   [14] work items   [15] bytes of column values the launch
+ *   reads: scan images where the staged loads take them, verbatim element bytes elsewhere (NULL words, deltas and
+ *   dictionaries not counted)
  * The first SDX_LAUNCH_LOG_MAX launches are kept.  *n = launches kept; min(cap, *n) records are written to out;
  * SD_ERR_OVERFLOW when cap < *n. */
 #define SDX_LAUNCH_WORDS 16

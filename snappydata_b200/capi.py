@@ -276,6 +276,10 @@ def product_api() -> Api:
         L.sdx_store_batch_info.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
         L.sdx_store_memory_info.restype = C.c_int
         L.sdx_store_memory_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.sdx_store_image_info.restype = C.c_int
+        L.sdx_store_image_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+        L.sdx_image_width.restype = C.c_int
+        L.sdx_image_width.argtypes = [C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_int64, C.POINTER(C.c_int32)]
         L.sdx_store_get_delta.restype = C.c_int
         L.sdx_store_get_delta.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
         L.sdx_store_get_deletes.restype = C.c_int
@@ -587,7 +591,7 @@ class Plan:
             out.append({"accumulator": LAUNCH_ACCUMULATORS[w[0]], "full_paths": bool(w[1]), "literal_nulls": bool(w[2]),
                         "nstages": w[3], "tile_rows": w[4], "chunk_rows": w[5], "grid": w[6], "ngroups": w[7],
                         "paths": dict(zip(BATCH_PATHS, w[8:12])), "replay": LAUNCH_REPLAYS[w[12]],
-                        "nbatches": w[13], "chunks": w[14]})
+                        "nbatches": w[13], "chunks": w[14], "streamed_bytes": w[15]})
         return out
 
     def set_option(self, option: int, value: int):
@@ -747,6 +751,12 @@ class Store:
         self.api.check(self.api.lib.sdx_store_memory_info(self.h, C.byref(comp), C.byref(total)))
         return comp.value, total.value
 
+    def image_info(self) -> Dict[str, int]:
+        """Scan images of the current batch versions (sdx_store_image_info)."""
+        out = (C.c_int64 * 4)()
+        self.api.check(self.api.lib.sdx_store_image_info(self.h, out))
+        return {"bytes": out[0], "images": out[1], "mismatches": out[2], "build_us": out[3]}
+
     def close(self):
         if self.h:
             self.api.store_destroy(self.h)
@@ -821,3 +831,10 @@ def last_reclaim_timing(api: Api) -> Dict[str, float]:
     out = (C.c_double * 6)()
     api.check(api.lib.sdx_last_reclaim_timing(out))
     return dict(zip(("plan_ms", "copy_ms", "install_ms", "free_ms", "reclaim_ms", "rounds"), list(out)))
+
+
+def image_width(api: Api, dict_image: bool, elem_bytes: int, ndistinct: int = 0, lo: int = 0, hi: int = 0) -> int:
+    """Width in bytes (0: none) of the scan image the store builds for one column of one batch (sdx_image_width)."""
+    w = C.c_int32()
+    api.check(api.lib.sdx_image_width(1 if dict_image else 0, elem_bytes, ndistinct, lo, hi, C.byref(w)))
+    return w.value

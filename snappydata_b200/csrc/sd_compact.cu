@@ -300,6 +300,11 @@ int compact_round(sd_store* s, cudaStream_t st, cudaEvent_t* ev, std::vector<Bat
   cudaEventElapsedTime(&c, ev[3], ev[4]);
   g_timing.mat_ms += a;
   g_timing.enc_ms += b + c;
+  {   // scan images of the rewritten columns (the kept ones keep theirs)
+    std::vector<StoredBatch*> fresh_nbs;
+    for (auto& nb : nbs) fresh_nbs.push_back(nb.get());
+    if ((rc = build_images(s, st, fresh_nbs, false))) return rc;
+  }
   for (size_t r = 0; r < round.size(); r++) {   // the rewritten columns' entries replace theirs; every other entry is kept as it is
     std::vector<std::pair<int, const ColStat*>> repl;
     for (size_t q = 0; q < round[r]->cols.size(); q++) repl.emplace_back(round[r]->cols[q].table_col, &stats[r][q]);

@@ -89,7 +89,18 @@ struct DevCol {
   int32_t enc;
   int32_t dict_n;             // dictionary entries (NULL code == dict_n for nullable columns)
   int32_t nruns;
+  // scan image (sd_image.cu): the same values as `data`, narrower, built and verified on the device when the batch version
+  // was created; only the staged loads read it.  Floating-point kinds: 1-byte indexes into img_tab, the distinct bit
+  // patterns (<= IMG_DICT_MAX).  Integral kinds and dictionary codes: unsigned offsets from img_tab[0] (frame of reference).
+  const uint8_t* img;         // img_w bytes per row, 128-byte aligned, or nullptr
+  const uint64_t* img_tab;
+  int32_t img_w;              // 1 or 2
+  int32_t img_n;              // words of img_tab (dictionary entries; 1 for a frame of reference)
 };
+
+constexpr int IMG_DICT_MAX = 256;
+// words of the scan kernel's per-chunk shared-memory copy of a column's img_tab
+constexpr int img_smem_words(int k) { return (k == K_F64 || k == K_F32) ? IMG_DICT_MAX : (k == K_BOOL || k == K_I8) ? 0 : 1; }
 
 template <int NC>
 struct DevBatch {
@@ -194,6 +205,8 @@ struct ScanArgs {
                                   // identity upload, one dependent operation less in front of the kernel)
   int32_t shift_cache_off;        // MODE_GROUPS with moment aggregates, TABLE_PRIVATE / TABLE_SHARED_ATOMIC: byte offset in
                                   // dynamic shared memory of the CTA's copy of the K words, [ngroups][NSHIFT]; -1: none
+  int32_t img_off;                // byte offset in dynamic shared memory of the per-chunk copies of the columns' img_tab
+                                  // (img_smem_words per column); -1: the staged loads read the verbatim values
   Literals lits;
 };
 

@@ -537,6 +537,10 @@ extern "C" int sd_store_encode_batch(sd_store* s, int32_t num_rows, const sd_raw
   sb->stats_ncols = (int32_t)s->schema.size();
   SD_CUDA(cudaStreamSynchronize(st));   // bodies written, side uploads done (ordered above): the batch may become visible
   {
+    int rc = build_images(s, st, {sb.get()}, false);
+    if (rc) return rc;
+  }
+  {
     std::lock_guard<std::mutex> lock(s->mu);
     s->batches.push_back(std::move(sb));
     s->version++;

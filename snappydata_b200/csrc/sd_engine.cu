@@ -290,7 +290,11 @@ struct StatEval {
 }  // namespace
 
 // batches of one launch per decode path: BATCH_ALL_FAST, BATCH_FAST_NULLS, BATCH_FAST_OVERLAY, general per-row decode
-struct PathCounts { int32_t n[4] = {0, 0, 0, 0}; };
+struct PathCounts {
+  int32_t n[4] = {0, 0, 0, 0};
+  // bytes of column values the launch reads: [0] every column verbatim, [1] scan images where the staged loads take them
+  int64_t streamed[2] = {0, 0};
+};
 
 // =====================================================================================================
 struct sd_plan {
@@ -531,6 +535,9 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
   const int nc = (int)sp.cols.size();
   const size_t bstride = sizeof(DevBatch<1>) - sizeof(DevCol) + (size_t)std::max(nc, 1) * sizeof(DevCol);
   const int nt = (int)sp.tables.size();
+  // SD_TUNE_NO_SCAN_IMAGES=1: the staged loads read the verbatim values (read per build, so one process can compare both)
+  const char* no_img_env = getenv("SD_TUNE_NO_SCAN_IMAGES");
+  const bool use_images = p->kernel.staged && !(no_img_env && atoi(no_img_env) > 0);
   std::vector<uint8_t> hb(bstride * std::max<size_t>(list.size(), 1), 0);
   std::vector<int32_t> prefix(list.size() + 1, 0);
   std::vector<uint8_t> aux;
@@ -555,6 +562,13 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
       const StoredCol& sc = sb.cols[t];
       if (!sc.unsupported.empty()) return set_error(SD_ERR_UNSUPPORTED, "column %d: %s", t, sc.unsupported.c_str());
       dc[c] = sc.dev;
+      {   // the scan image, when the kernel's decode of this column's kind reproduces the verbatim element from it
+        const int k = sp.kinds[c];
+        const bool match = sc.img_dict ? ((k == K_F64 && sc.img_ew == 8) || (k == K_F32 && sc.img_ew == 4))
+                                       : ((k == K_I64 && sc.img_ew == 8) || (k == K_I32 && sc.img_ew == 4) || (k == K_I16 && sc.img_ew == 2) ||
+                                          (k == K_CODE && ((sc.dev.enc == ENC_DICTIONARY && sc.img_ew == 2) || (sc.dev.enc == ENC_BIG_DICTIONARY && sc.img_ew == 4))));
+        if (!(use_images && sc.dev.img && match && !sc.has_nulls)) { dc[c].img = nullptr; dc[c].img_tab = nullptr; dc[c].img_w = 0; dc[c].img_n = 0; }
+      }
       all_fast = all_fast && sc.fast;
       {
         const bool simple = (sp.kinds[c] == K_CODE && (sc.dev.enc == ENC_DICTIONARY || sc.dev.enc == ENC_BIG_DICTIONARY || sc.dev.enc == ENC_STR_RAW)) ||
@@ -572,6 +586,12 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
     hdr->flags = all_fast ? BATCH_ALL_FAST : (base_fast ? BATCH_FAST_OVERLAY : ((simple_enc && !any_delta && !sb.dev_deletes) ? BATCH_FAST_NULLS : 0));
     if (!(hdr->flags == BATCH_ALL_FAST || (hdr->flags == BATCH_FAST_NULLS && p->kernel.staged))) out->needs_slow = 1;
     out->paths.n[hdr->flags == BATCH_ALL_FAST ? 0 : hdr->flags == BATCH_FAST_NULLS ? 1 : hdr->flags == BATCH_FAST_OVERLAY ? 2 : 3]++;
+    for (int c = 0; c < nc; c++) {   // only the staged loads of the staged-only kernel variant read images (launch_scan)
+      const int k = sp.kinds[c];
+      const int64_t verbatim = k == K_CODE ? (dc[c].enc == ENC_DICTIONARY ? 2 : 4) : kind_stage_width(k);
+      out->paths.streamed[0] += verbatim * sb.num_rows;
+      out->paths.streamed[1] += (hdr->flags && dc[c].img ? dc[c].img_w : verbatim) * sb.num_rows;
+    }
     // per-batch tables: [int32 offset x nt][pad 8][uint64 kpack x nt][tables]; every table is indexed by the
     // unified dictionary code; key maps of <= 8 codes are also packed one byte per code into kpack
     if (nt) {
@@ -876,7 +896,19 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
     if (nshift > 0 && table_mode != TABLE_GLOBAL_ATOMIC) shift_cache_off = (int)(tile_smem + table_bytes - kc);
   }
   const size_t budget = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
-  size_t ring_off = (tile_smem + table_bytes + 127) & ~size_t(127);
+  // the per-chunk copies of the image tables sit between the group table and the ring, when the batches have images, the
+  // kernel is the staged-only variant (the one with the per-row paths reads verbatim values) and the ring keeps at least
+  // two stages
+  int img_off = -1;
+  size_t img_end = tile_smem + table_bytes;
+  const bool slow_variant = k == &p->variant[2] || k == &p->variant[3];
+  if (k->staged && !slow_variant && paths.streamed[1] < paths.streamed[0]) {
+    size_t img_bytes = 0;
+    for (int kd : sp.kinds) img_bytes += 8 * (size_t)img_smem_words(kd);
+    const size_t off = (tile_smem + table_bytes + 15) & ~size_t(15);
+    if (((off + img_bytes + 127) & ~size_t(127)) + min_ring <= budget) { img_off = (int)off; img_end = off + img_bytes; }
+  }
+  size_t ring_off = (img_end + 127) & ~size_t(127);
   int nstages = 0;
   size_t smem = ring_off;
   if (k->staged) {
@@ -951,6 +983,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   args.chunk_rows = p->chunk_rows;
   args.fresh = fresh;
   args.shift_cache_off = shift_cache_off;
+  args.img_off = img_off;
   memcpy(args.radix, radix, sizeof(radix));
   if (p->litpool_dirty) {   // STRING literal bytes -> device (once per set of literal values)
     std::vector<uint8_t> pool;
@@ -1004,7 +1037,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
                   : table_mode == TABLE_GLOBAL_ATOMIC ? SDX_ACC_GLOBAL_ATOMIC : SDX_ACC_REGTABLE;
     const int64_t rec[SDX_LAUNCH_WORDS] = {acc, k == &p->variant[2] || k == &p->variant[3], k == &p->variant[1] || k == &p->variant[3],
                                            nstages, k->tile_rows, p->chunk_rows, grid, ngroups, paths.n[0], paths.n[1], paths.n[2],
-                                           paths.n[3], p->replay_kind, nbatches, total_chunks, 0};
+                                           paths.n[3], p->replay_kind, nbatches, total_chunks, paths.streamed[img_off >= 0 ? 1 : 0]};
     p->launch_records.insert(p->launch_records.end(), rec, rec + SDX_LAUNCH_WORDS);
   }
   SD_CUDA(cudaEventRecord(p->ev_stop, p->stream));

@@ -162,6 +162,7 @@ extern "C" int sdx_store_gen_lineitem(sd_store* s, int64_t first_row, int64_t nr
   static const char* ls_str[2] = {"O", "F"};
   std::vector<GenBatch> gen(nb);
   const size_t first_batch = s->batches.size();
+  std::vector<StoredBatch*> fresh;
   for (int b = 0; b < nb; b++) {
     GenBatch& g = gen[b];
     memset(&g, 0, sizeof(g));
@@ -222,6 +223,7 @@ extern "C" int sdx_store_gen_lineitem(sd_store* s, int64_t first_row, int64_t nr
       g.col[k] = c.dev_base;
       g.body_off[k] = body;
     }
+    fresh.push_back(sb.get());
     s->batches.push_back(std::move(sb));
   }
   (void)first_batch;
@@ -230,6 +232,7 @@ extern "C" int sdx_store_gen_lineitem(sd_store* s, int64_t first_row, int64_t nr
   SD_CUDA(cudaGetLastError());
   SD_CUDA(cudaStreamSynchronize(s->copy_stream));
   cudaFree(d_firsts); cudaFree(d_counts); cudaFree(d_first_seen); cudaFree(d_prefix); cudaFree(d_gen);
+  { int rc = build_images(s, s->copy_stream, fresh, true); if (rc) return rc; }
   s->version++;
   return 0;
 }

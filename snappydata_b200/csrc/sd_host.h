@@ -179,6 +179,11 @@ struct StoredCol {
   StoredDelta delta[2];
   DevDelta* dev_delta[2] = {nullptr, nullptr};   // DevDelta structs resident on the device
   bool fast = false;                      // vector fast path applies
+  // scan image (sd_image.cu; DevCol.img): element bytes of the verbatim values it reproduces, whether it is a dictionary of
+  // bit patterns (else a frame of reference), and the arena bytes it takes
+  int32_t img_ew = 0;
+  bool img_dict = false;
+  int64_t img_bytes = 0;
 };
 
 inline uint64_t next_batch_uid() { static std::atomic<uint64_t> n{1}; return n.fetch_add(1, std::memory_order_relaxed); }
@@ -223,6 +228,8 @@ void visit_device_pointers(StoredBatch& b, F&& f) {
     one(sc.dev.run_ends, c, "run_ends");
     one(sc.dev.delta0, c, "delta0");
     one(sc.dev.delta1, c, "delta1");
+    one(sc.dev.img, c, "img");
+    one(sc.dev.img_tab, c, "img_tab");
     for (int d = 0; d < 2; d++) {
       StoredDelta& sd = sc.delta[d];
       if (sd.present) {
@@ -237,6 +244,15 @@ void visit_device_pointers(StoredBatch& b, F&& f) {
   }
   one(b.dev_deletes, -1, "dev_deletes");
 }
+// Scan images of the given fresh batch versions (sd_image.cu): every NOT NULL column without NULLs in the batch whose values
+// fit a narrower byte-aligned form gets one, built and verified on the device, placed in the store's arena as extents of its
+// version.  Columns that already have an image keep it.  The batches' bytes are complete in stream order on `st`; the
+// batches are not yet visible to scans.  `locked`: the caller holds s->mu (else it is taken for the arena placement only,
+// so that scans are not held up by the build).  Synchronises `st`.
+int build_images(sd_store* s, cudaStream_t st, const std::vector<StoredBatch*>& batches, bool locked);
+// image choice for a column's values: width in bytes (0: none) of a dictionary image (float kinds, `ndistinct` distinct bit
+// patterns) or a frame of reference over [lo, hi] (integral kinds, element width ew)
+int image_width(bool dict, int ew, uint64_t ndistinct, int64_t lo, int64_t hi);
 // drop the extents no device pointer of the version lies in (those a replaced delta / mask / column left behind)
 void prune_extents(StoredBatch& b);
 
@@ -319,11 +335,16 @@ struct sd_store {
   std::mutex enc_mu;               // one encoder at a time per store; `mu` is taken only to lay the buffers out and to publish
   cudaStream_t enc_stream = nullptr;
   cudaEvent_t enc_event = nullptr;   // page-locked copies of the job lists (a pageable source would stall the caller per flush)
+  // scan images (sd_image.cu): (batch, column) images whose device verification failed (the column keeps its verbatim path),
+  // and the time spent building images
+  int64_t image_mismatches = 0;
+  double image_ms = 0;
 };
 
 namespace sd {
-// upload one batch (columns by table ordinal of `schema`) into the store's arena
-int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals /* nullptr: identity */);
+// upload one batch (columns by table ordinal of `schema`) into the store's arena; `images`: build its scan images (resident
+// stores; the private store of sd_batch_submit scans each batch once and skips them)
+int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals /* nullptr: identity */, bool images = false);
 // queue the expansion of every pending compressed buffer (asynchronous; no-op when nothing is pending)
 int store_flush_lz4(sd_store* s);
 // make `stream` wait for every expansion queued so far

@@ -809,13 +809,20 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 // consumer-only CTA barrier (the producer warp never joins it)
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(THREADS) : "memory"); }
 
-// byte offset of column C's tile inside a stage
+// byte offset of column C's tile inside a stage (sized by the verbatim width: a scan image is never wider)
 template <class PLAN>
 __host__ __device__ constexpr int stage_col_off(int c) {
   int off = 0;
   // + 128: a column with NULLs is copied from the 16-byte boundary below its first value of the tile (<= 15 extra
   // bytes); a full 128 keeps every column's region 128-byte aligned for the bulk copies
   for (int i = 0; i < c; i++) off += THREADS * PLAN::RPT * kind_stage_width(PLAN::kind(i)) + 128;
+  return off;
+}
+// word offset of column C's img_tab copy in the kernel's shared-memory image tables (ScanArgs.img_off)
+template <class PLAN>
+__host__ __device__ constexpr int img_col_off(int c) {
+  int off = 0;
+  for (int i = 0; i < c; i++) off += img_smem_words(PLAN::kind(i));
   return off;
 }
 template <class PLAN>
@@ -828,10 +835,21 @@ template <bool WIDE> struct CMaskT { typedef uint32_t T; };
 template <> struct CMaskT<true> { typedef uint64_t T; };
 #define SD_CMASK(PLAN) typename CMaskT<(PLAN::NC > 32)>::T
 
-// element width of column C in this batch (dictionary indexes are int16 or int32)
+// what the staged loads of one batch read, one bit per column (uniform per work item)
+template <class PLAN>
+struct ColModes {
+  typedef SD_CMASK(PLAN) M;
+  M c16;      // K_CODE column with int16 dictionary indexes (else int32)
+  M img;      // the column's scan image (DevCol.img) instead of its verbatim values
+  M w1;       // image width 1 (else 2)
+};
+__host__ __device__ constexpr bool kind_has_image(int k) { return k != K_BOOL && k != K_I8; }
+
+// element width of column C in this batch (dictionary indexes are int16 or int32; images 1 or 2 bytes)
 template <class PLAN, int C>
-__device__ __forceinline__ int col_width(SD_CMASK(PLAN) c16) {
-  return PLAN::kind(C) == K_CODE ? (((c16 >> C) & 1) ? 2 : 4) : (int)sizeof(typename KindT<PLAN::kind(C)>::T);
+__device__ __forceinline__ int col_width(const ColModes<PLAN>& cm) {
+  if (kind_has_image(PLAN::kind(C)) && ((cm.img >> C) & 1)) return ((cm.w1 >> C) & 1) ? 1 : 2;
+  return PLAN::kind(C) == K_CODE ? (((cm.c16 >> C) & 1) ? 2 : 4) : (int)sizeof(typename KindT<PLAN::kind(C)>::T);
 }
 
 // per-chunk copy of the descriptor fields the producer needs (with the SM's shared memory carved out for the ring
@@ -842,8 +860,9 @@ struct ProducerCols {
   const int32_t* tile_nulls[NC > 0 ? NC : 1];
 };
 template <class PLAN, int... Cs>
-__device__ __forceinline__ void load_producer_cols(const DevBatch<PLAN::NC>& b, ProducerCols<PLAN::NC>& pc, Seq<Cs...>) {
-  int dummy[] = {0, (pc.data[Cs] = b.cols[Cs].data, pc.tile_nulls[Cs] = PLAN::col_nullable(Cs) ? b.cols[Cs].tile_nulls : nullptr, 0)...};
+__device__ __forceinline__ void load_producer_cols(const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, ProducerCols<PLAN::NC>& pc, Seq<Cs...>) {
+  int dummy[] = {0, (pc.data[Cs] = ((cm.img >> Cs) & 1) ? b.cols[Cs].img : b.cols[Cs].data,
+                     pc.tile_nulls[Cs] = PLAN::col_nullable(Cs) ? b.cols[Cs].tile_nulls : nullptr, 0)...};
   (void)dummy;
 }
 
@@ -851,8 +870,8 @@ __device__ __forceinline__ void load_producer_cols(const DevBatch<PLAN::NC>& b, 
 // ordinal; with NULLs the tile's stored values are [tile_start - nulls_before(tile_start), ... ) and their count is
 // rows - nulls_in_tile, both from the host-computed prefix (one entry per NULL_PREFIX_ROWS rows)
 template <class PLAN, int C>
-__device__ __forceinline__ void col_copy_range(const int32_t* tile_nulls, SD_CMASK(PLAN) c16, int64_t tile_start, int rows, int64_t* src_off, uint32_t* bytes) {
-  const int w = col_width<PLAN, C>(c16);
+__device__ __forceinline__ void col_copy_range(const int32_t* tile_nulls, const ColModes<PLAN>& cm, int64_t tile_start, int rows, int64_t* src_off, uint32_t* bytes) {
+  const int w = col_width<PLAN, C>(cm);
   int64_t first = tile_start;
   int cnt = rows;
   if (PLAN::col_nullable(C) && tile_nulls) {
@@ -866,29 +885,50 @@ __device__ __forceinline__ void col_copy_range(const int32_t* tile_nulls, SD_CMA
   *bytes = cnt > 0 ? (uint32_t)(((off & 15) + (int64_t)cnt * w + 15) & ~int64_t(15)) : 0u;   // buffers are padded: over-reading is safe
 }
 template <class PLAN, int... Cs>
-__device__ __forceinline__ void issue_tile_copies(const ProducerCols<PLAN::NC>& pc, SD_CMASK(PLAN) c16, int64_t tile_start, int rows, uint8_t* stage, uint64_t* bar, Seq<Cs...>) {
+__device__ __forceinline__ void issue_tile_copies(const ProducerCols<PLAN::NC>& pc, const ColModes<PLAN>& cm, int64_t tile_start, int rows, uint8_t* stage, uint64_t* bar, Seq<Cs...>) {
   int64_t off[PLAN::NC > 0 ? PLAN::NC : 1];
   uint32_t bytes[PLAN::NC > 0 ? PLAN::NC : 1];
   uint32_t total = 0;
-  int d0[] = {0, (col_copy_range<PLAN, Cs>(pc.tile_nulls[Cs], c16, tile_start, rows, &off[Cs], &bytes[Cs]), total += bytes[Cs], 0)...};
+  int d0[] = {0, (col_copy_range<PLAN, Cs>(pc.tile_nulls[Cs], cm, tile_start, rows, &off[Cs], &bytes[Cs]), total += bytes[Cs], 0)...};
   (void)d0;
   mbar_expect_tx(bar, total);
   int d1[] = {0, ((!PLAN::col_nullable(Cs) || bytes[Cs]) ? (bulk_g2s(stage + stage_col_off<PLAN>(Cs), pc.data[Cs] + off[Cs], bytes[Cs], bar), 0) : 0)...};
   (void)d1;
 }
 
+// value of image code x: dictionary entry (floating-point kinds) or frame-of-reference offset, from the chunk's shared copy
+template <int K, class T>
+__device__ __forceinline__ T img_value(const uint64_t* tab, uint32_t x) {
+  if (K == K_F64) return (T)__longlong_as_double((long long)tab[x]);
+  if (K == K_F32) return (T)__int_as_float((int)(uint32_t)tab[x]);
+  return (T)((int64_t)tab[0] + (int64_t)x);   // wraps to the element width exactly as the image builder verified
+}
 // consumer: registers <- stage (conflict-free: consecutive lanes read consecutive 16/8/4/2 bytes)
 template <class PLAN, int C>
-__device__ __forceinline__ void load_col_staged(SD_CMASK(PLAN) c16, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
+__device__ __forceinline__ void load_col_staged(const ColModes<PLAN>& cm, const uint64_t* imgsm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
   typedef typename KindT<PLAN::kind(C)>::T T;
   constexpr int K = PLAN::kind(C);
   const uint8_t* base = stage + stage_col_off<PLAN>(C);
   regs.nullmask = 0;
+  if (kind_has_image(K) && ((cm.img >> C) & 1)) {
+    const uint64_t* tab = imgsm + img_col_off<PLAN>(C);
+    const bool w1 = (cm.w1 >> C) & 1;
+#pragma unroll
+    for (int u = 0; u < PLAN::RPT / 2; u++) {
+      const int p = u * 2 * THREADS + 2 * (int)threadIdx.x;
+      uint32_t x0, x1;
+      if (w1) { const uint32_t x = *reinterpret_cast<const uint16_t*>(base + p); x0 = x & 0xffu; x1 = x >> 8; }
+      else { const uint32_t x = *reinterpret_cast<const uint32_t*>(base + p * 2); x0 = x & 0xffffu; x1 = x >> 16; }
+      regs.v[2 * u] = img_value<K, T>(tab, x0);
+      regs.v[2 * u + 1] = img_value<K, T>(tab, x1);
+    }
+    return;
+  }
 #pragma unroll
   for (int u = 0; u < PLAN::RPT / 2; u++) {
     const int p = u * 2 * THREADS + 2 * (int)threadIdx.x;
     if (K == K_CODE) {
-      if ((c16 >> C) & 1) {
+      if ((cm.c16 >> C) & 1) {
         uint32_t x = *reinterpret_cast<const uint32_t*>(base + p * 2);
         regs.v[2 * u] = (T)(int16_t)(x & 0xffffu);
         regs.v[2 * u + 1] = (T)(int16_t)(x >> 16);
@@ -919,11 +959,11 @@ __device__ __forceinline__ void load_col_staged(SD_CMASK(PLAN) c16, const uint8_
 // consumer, column with NULLs: row -> (is null, value index) through the null words; the value sits in the stage at
 // [shift + (k - first) * w] where `first` is the tile's first stored value
 template <class PLAN, int C>
-__device__ __forceinline__ void load_col_staged_nulls(const DevCol& col, SD_CMASK(PLAN) c16, int64_t tile_start, int num_rows,
+__device__ __forceinline__ void load_col_staged_nulls(const DevCol& col, const ColModes<PLAN>& cm, int64_t tile_start, int num_rows,
                                                       const TileSmem<PLAN>& sm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
   typedef typename KindT<PLAN::kind(C)>::T T;
   constexpr int K = PLAN::kind(C);
-  const int w = col_width<PLAN, C>(c16);
+  const int w = col_width<PLAN, C>(cm);   // (a column with NULLs in the batch has no image)
   const int n0 = col.tile_nulls[tile_start / NULL_PREFIX_ROWS];
   const int64_t first = tile_start - n0;
   const uint8_t* base = stage + stage_col_off<PLAN>(C) + ((first * w) & 15);
@@ -965,20 +1005,20 @@ __device__ __forceinline__ void load_col_staged_nulls(const DevCol& col, SD_CMAS
   }
 }
 template <class PLAN, int C>
-__device__ __forceinline__ void load_col_staged_any(const DevCol& col, SD_CMASK(PLAN) c16, int64_t tile_start, int num_rows,
+__device__ __forceinline__ void load_col_staged_any(const DevCol& col, const ColModes<PLAN>& cm, const uint64_t* imgsm, int64_t tile_start, int num_rows,
                                                     const TileSmem<PLAN>& sm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
-  if (PLAN::col_nullable(C) && col.nulls) load_col_staged_nulls<PLAN, C>(col, c16, tile_start, num_rows, sm, stage, regs);
-  else load_col_staged<PLAN, C>(c16, stage, regs);
+  if (PLAN::col_nullable(C) && col.nulls) load_col_staged_nulls<PLAN, C>(col, cm, tile_start, num_rows, sm, stage, regs);
+  else load_col_staged<PLAN, C>(cm, imgsm, stage, regs);
 }
 template <class PLAN, int... Cs>
-__device__ __forceinline__ void load_all_staged_nulls(const DevBatch<PLAN::NC>& b, SD_CMASK(PLAN) c16, int64_t tile_start, const TileSmem<PLAN>& sm,
+__device__ __forceinline__ void load_all_staged_nulls(const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, const uint64_t* imgsm, int64_t tile_start, const TileSmem<PLAN>& sm,
                                                       const uint8_t* stage, AllCols<PLAN, Seq<Cs...>>& regs, Seq<Cs...>) {
-  int dummy[] = {0, (load_col_staged_any<PLAN, Cs>(b.cols[Cs], c16, tile_start, b.num_rows, sm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
+  int dummy[] = {0, (load_col_staged_any<PLAN, Cs>(b.cols[Cs], cm, imgsm, tile_start, b.num_rows, sm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
   (void)dummy;
 }
 template <class PLAN, int... Cs>
-__device__ __forceinline__ void load_all_staged(SD_CMASK(PLAN) c16, const uint8_t* stage, AllCols<PLAN, Seq<Cs...>>& regs, Seq<Cs...>) {
-  int dummy[] = {0, (load_col_staged<PLAN, Cs>(c16, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
+__device__ __forceinline__ void load_all_staged(const ColModes<PLAN>& cm, const uint64_t* imgsm, const uint8_t* stage, AllCols<PLAN, Seq<Cs...>>& regs, Seq<Cs...>) {
+  int dummy[] = {0, (load_col_staged<PLAN, Cs>(cm, imgsm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
   (void)dummy;
 }
 
@@ -1041,14 +1081,28 @@ __device__ __forceinline__ void load_strbase(RowCtx& ctx, const DevBatch<PLAN::N
   (void)dummy;
 }
 
-// bit c set: K_CODE column c of this batch uses int16 dictionary indexes (else int32)
+// what the staged loads of batch b read (images only when the launch has room for their tables: with_img; never in the
+// variant with the per-row paths, whose register budget they would take)
 template <class PLAN, int... Cs>
-__device__ __forceinline__ SD_CMASK(PLAN) code16_mask(const DevBatch<PLAN::NC>& b, Seq<Cs...>) {
+__device__ __forceinline__ ColModes<PLAN> col_modes(const DevBatch<PLAN::NC>& b, bool with_img, Seq<Cs...>) {
   typedef SD_CMASK(PLAN) M;
-  M m = 0;
-  int dummy[] = {0, (PLAN::kind(Cs) == K_CODE ? (m |= (M)(b.cols[Cs].enc == ENC_DICTIONARY ? 1 : 0) << Cs, 0) : 0)...};
+  ColModes<PLAN> cm;
+  cm.c16 = 0; cm.img = 0; cm.w1 = 0;
+  int dummy[] = {0, (PLAN::kind(Cs) == K_CODE ? (cm.c16 |= (M)(b.cols[Cs].enc == ENC_DICTIONARY ? 1 : 0) << Cs, 0) : 0)...};
+  if (PLAN::STAGES > 0 && !PLAN::SLOW_PATHS && with_img) {
+    int d1[] = {0, (kind_has_image(PLAN::kind(Cs)) && b.cols[Cs].img
+                    ? (cm.img |= (M)1 << Cs, cm.w1 |= (M)(b.cols[Cs].img_w == 1) << Cs, 0) : 0)...};
+    (void)d1;
+  }
   (void)dummy;
-  return m;
+  return cm;
+}
+// the chunk's img_tab words -> shared memory (the caller brackets this with consumer barriers)
+template <class PLAN, int... Cs>
+__device__ __forceinline__ void load_img_tables(const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, uint64_t* imgsm, Seq<Cs...>) {
+  int dummy[] = {0, (kind_has_image(PLAN::kind(Cs)) && ((cm.img >> Cs) & 1)
+                     ? ([&] { for (int i = threadIdx.x; i < b.cols[Cs].img_n; i += THREADS) imgsm[img_col_off<PLAN>(Cs) + i] = __ldg(&b.cols[Cs].img_tab[i]); }(), 0) : 0)...};
+  (void)dummy;
 }
 
 // ================================================================================================
@@ -1098,14 +1152,14 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
           const int num_rows = b.num_rows;
           const int ntiles = (num_rows + TILE_ROWS - 1) / TILE_ROWS;
           const int tile0 = chunk * CHUNK_TILES, tile_end = min(tile0 + CHUNK_TILES, ntiles);
-          const SD_CMASK(PLAN) c16 = code16_mask<PLAN>(b, ColSeq());
+          const ColModes<PLAN> cm = col_modes<PLAN>(b, args.img_off >= 0, ColSeq());
           ProducerCols<PLAN::NC> pc;
-          load_producer_cols<PLAN>(b, pc, ColSeq());
+          load_producer_cols<PLAN>(b, cm, pc, ColSeq());
           for (int tile = tile0; tile < tile_end; tile++) {
             const int64_t tile_start = (int64_t)tile * TILE_ROWS;
             const int rows = min(TILE_ROWS, num_rows - (int)tile_start);
             mbar_wait(&empty_bar[stage], phase ^ 1u);
-            issue_tile_copies<PLAN>(pc, c16, tile_start, rows, ring + (size_t)stage * StageInfo<PLAN>::BYTES, &full_bar[stage], ColSeq());
+            issue_tile_copies<PLAN>(pc, cm, tile_start, rows, ring + (size_t)stage * StageInfo<PLAN>::BYTES, &full_bar[stage], ColSeq());
             if (++stage == nstages) { stage = 0; phase ^= 1u; }
           }
         }
@@ -1116,6 +1170,9 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   int c_stage = 0;
   uint32_t c_phase = 0;
   int c_hint = -1;
+  // per-chunk shared copies of the image tables (at args.img_off); refreshed when a work item's batch differs from the
+  // last one loaded
+  int img_batch = -1;
 
   // ---- accumulator init -------------------------------------------------------------------------
   uint64_t acc[NSLOT > 0 ? NSLOT : 1];
@@ -1177,7 +1234,13 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     if (!PLAN::SLOW_PATHS && !fast) __trap();
     load_tables<PLAN::NTABLES>(ctx, b.aux);
     if (PLAN::ANY_STRING) load_strbase<PLAN>(ctx, b, ColSeq());
-    const SD_CMASK(PLAN) c16 = code16_mask<PLAN>(b, ColSeq());
+    const ColModes<PLAN> cm = col_modes<PLAN>(b, args.img_off >= 0, ColSeq());
+    if (PLAN::STAGES > 0 && !PLAN::SLOW_PATHS && fast && cm.img && lo != img_batch) {
+      consumer_sync();   // every consumer is done with the previous batch's tables
+      load_img_tables<PLAN>(b, cm, reinterpret_cast<uint64_t*>(smem_raw + args.img_off), ColSeq());
+      consumer_sync();
+      img_batch = lo;
+    }
     uint32_t c_scanned = 0, c_passed = 0;
     const int tile0 = chunk * CHUNK_TILES;
     const int ntiles = (num_rows + TILE_ROWS - 1) / TILE_ROWS;
@@ -1193,8 +1256,9 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
       if (fast) {
         if (PLAN::STAGES > 0) {
           mbar_wait(&full_bar[c_stage], c_phase);   // (the NULL-aware loads derive their word prefixes per warp: no barrier here)
-          if (with_nulls) load_all_staged_nulls<PLAN>(b, c16, tile_start, sm, ring + (size_t)c_stage * StageInfo<PLAN>::BYTES, regs, ColSeq());
-          else load_all_staged<PLAN>(c16, ring + (size_t)c_stage * StageInfo<PLAN>::BYTES, regs, ColSeq());
+          const uint64_t* imgsm = reinterpret_cast<const uint64_t*>(smem_raw + args.img_off);   // (read only where cm.img)
+          if (with_nulls) load_all_staged_nulls<PLAN>(b, cm, imgsm, tile_start, sm, ring + (size_t)c_stage * StageInfo<PLAN>::BYTES, regs, ColSeq());
+          else load_all_staged<PLAN>(cm, imgsm, ring + (size_t)c_stage * StageInfo<PLAN>::BYTES, regs, ColSeq());
           // The rows of this tile are in registers now: release the stage.  The stage was read through the GENERIC proxy (ld.shared)
           // and will be refilled through the ASYNC proxy (cp.async.bulk): the mbarrier alone does not order the two (PTX ISA, "async
           // proxy": accesses to the same location across proxies need a cross-proxy fence).  Without the fence a refill can land

@@ -753,7 +753,7 @@ int store_lz4_check(sd_store* s) {
   return 0;
 }
 
-int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals) {
+int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals, bool images) {
   if (!b || b->num_rows < 0) return set_error(SD_ERR_INVALID, "bad batch");
   std::lock_guard<std::mutex> lock(s->mu);
   cudaSetDevice(s->device);
@@ -761,6 +761,7 @@ int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals) {
   sb->num_rows = b->num_rows; sb->bucket_id = b->bucket_id; sb->batch_id = b->batch_id;
   sb->cols.resize(s->schema.size());
   ExtentRecorder rec(s->arena, &sb->extents);   // every arena allocation of this put belongs to the new batch
+  const size_t lz4_before = s->pending_lz4.size();
   {   // LZ4 envelopes that lie (almost) back to back in host memory: one host->device copy for the lot (small copies reach
       // a lower link rate than large ones)
     s->span_h0 = nullptr;
@@ -892,6 +893,12 @@ int store_put(sd_store* s, const sd_batch* b, const int32_t* table_ordinals) {
   if (!s->retain_buffers) {
     SD_CUDA(cudaStreamSynchronize(s->copy_stream));
     for (int k = 0; k + 1 < s->num_copy_streams; k++) SD_CUDA(cudaStreamSynchronize(s->extra_streams[k]));
+    // scan images of a put whose bytes are all on the device now (one with LZ4 payloads still to expand keeps the verbatim
+    // path, as does an asynchronous put of retained buffers)
+    if (images && s->pending_lz4.size() == lz4_before) {
+      int rc = build_images(s, s->copy_stream, {sb.get()}, true);
+      if (rc) return rc;
+    }
   }
   s->batches.push_back(std::move(sb));
   s->version++;
@@ -958,7 +965,7 @@ int sd_store_create(int device, int32_t ncols, const sd_column* schema, sd_store
 int sd_store_put_batch(sd_store* s, const sd_batch* b) {
   if (!s || !b) return sd::set_error(SD_ERR_INVALID, "sd_store_put_batch: null argument");
   if (b->ncols != (int)s->schema.size()) return sd::set_error(SD_ERR_INVALID, "sd_store_put_batch: batch has %d columns, table schema %zu", b->ncols, s->schema.size());
-  return sd::store_put(s, b, nullptr);
+  return sd::store_put(s, b, nullptr, true);
 }
 
 int sd_store_num_batches(sd_store* s, int64_t* out) { std::lock_guard<std::mutex> lock(s->mu); *out = (int64_t)s->batches.size(); return 0; }
