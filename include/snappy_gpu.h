@@ -80,7 +80,9 @@ typedef enum sd_op {
   SD_OP_AND = 30, SD_OP_OR = 31, SD_OP_NOT = 32,
   SD_OP_ISNULL = 33, SD_OP_ISNOTNULL = 34,
   SD_OP_IN = 35,        /* a = expr, b = first literal slot, c = number of literals */
-  SD_OP_STARTSWITH = 36 /* a = string expr, b = literal node                     */
+  SD_OP_STARTSWITH = 36, /* a = string expr, b = literal node                    */
+  SD_OP_PAIR = 37       /* a = x node, b = y node, both DOUBLE; type DOUBLE, NULL when either is NULL.  Only as the input
+                           of a two-input aggregate (COVAR_POP / COVAR_SAMP / CORR); anywhere else SD_ERR_INVALID */
 } sd_op;
 
 typedef struct sd_expr {
@@ -127,11 +129,24 @@ typedef struct sd_expr {
  * SKEWNESS NaN when m2 == 0, else sqrt(n)*m3/sqrt(m2^3); KURTOSIS NaN when m2 == 0, else n*m4/m2^2 - 3.  A NaN or +-Inf input
  * makes the group's results NaN.  The device sums (x - K)^j around one shift K per group and input (the first value the group
  * sees) and the partial rows carry the buffers above; plans with moment aggregates have no dense partials export
- * (sd_plan_partials_layout / sd_plan_export_partials / sd_plan_import_partials: SD_ERR_UNSUPPORTED). */
+ * (sd_plan_partials_layout / sd_plan_export_partials / sd_plan_import_partials: SD_ERR_UNSUPPORTED).
+ * Two-input aggregates (Spark 2.1.1 Covariance / Corr, restated from upstream Spark; the fork's source is not at hand).  The
+ * input node must be an SD_OP_PAIR of two DOUBLE nodes (x, y), else SD_ERR_INVALID; a row counts only when both are non-null.
+ * Buffers are non-nullable DOUBLEs, 0.0 before any input, in aggBufferAttributes order:
+ *   COVAR_POP / COVAR_SAMP : [n, xAvg, yAvg, ck]
+ *   CORR                   : [n, xAvg, yAvg, ck, xMk, yMk]
+ * (ck = sum (x - xAvg)(y - yAvg), xMk = sum (x - xAvg)^2, yMk likewise).  Merge:
+ *   n = n1+n2, dx = xAvg2-xAvg1, dxN = n == 0 ? 0 : dx/n, dy / dyN likewise, xAvg = xAvg1 + dxN*n2, yAvg = yAvg1 + dyN*n2,
+ *   ck = ck1+ck2 + dx*dyN*n1*n2, xMk = xMk1+xMk2 + dx*dxN*n1*n2, yMk likewise.
+ * Results are DOUBLE, NULL when n == 0; COVAR_POP ck/n; COVAR_SAMP NaN when n == 1, else ck/(n-1); CORR NaN when n == 1, else
+ * ck/sqrt(xMk*yMk).  The device sums (x - Kx), (y - Ky), (x - Kx)(y - Ky) (and for CORR the squares) around one shift pair
+ * (Kx, Ky) per group and input pair.  A group in which a counted row has a NaN or +-Inf x or y gets NaN in every buffer but n,
+ * so its results are NaN (Spark's row-order update gives +-Inf or NaN there, depending on where the row falls).  Plans with
+ * these aggregates have no dense partials export either. */
 typedef enum sd_agg_fn {
   SD_AGG_COUNT_STAR = 1, SD_AGG_COUNT = 2, SD_AGG_SUM = 3, SD_AGG_AVG = 4, SD_AGG_MIN = 5, SD_AGG_MAX = 6,
   SD_AGG_STDDEV_POP = 7, SD_AGG_STDDEV_SAMP = 8, SD_AGG_VAR_POP = 9, SD_AGG_VAR_SAMP = 10, SD_AGG_SKEWNESS = 11,
-  SD_AGG_KURTOSIS = 12
+  SD_AGG_KURTOSIS = 12, SD_AGG_COVAR_POP = 13, SD_AGG_COVAR_SAMP = 14, SD_AGG_CORR = 15
 } sd_agg_fn;
 
 typedef struct sd_agg {

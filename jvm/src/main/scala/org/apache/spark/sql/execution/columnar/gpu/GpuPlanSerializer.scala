@@ -48,11 +48,14 @@ private[gpu] object Abi {
   final val EQ = 20; final val NE = 21; final val LT = 22; final val LE = 23; final val GT = 24; final val GE = 25
   final val AND = 30; final val OR = 31; final val NOT = 32; final val ISNULL = 33; final val ISNOTNULL = 34
   final val IN = 35; final val STARTSWITH = 36
+  final val PAIR = 37   // (x, y) input of COVAR_POP / COVAR_SAMP / CORR
   // sd_agg_fn
   final val COUNT_STAR = 1; final val COUNT = 2; final val SUM = 3; final val AVG = 4; final val MIN = 5; final val MAX = 6
   // CentralMomentAgg: the child is DOUBLE (ImplicitCastInputTypes puts a Cast in front of any other numeric input)
   final val STDDEV_POP = 7; final val STDDEV_SAMP = 8; final val VAR_POP = 9; final val VAR_SAMP = 10; final val SKEWNESS = 11
   final val KURTOSIS = 12
+  // Covariance / Corr: two DOUBLE children (ImplicitCastInputTypes casts them), sent as one PAIR node
+  final val COVAR_POP = 13; final val COVAR_SAMP = 14; final val CORR = 15
   // struct sizes / offsets (x86-64; jvm/abi_offsets.txt is generated from the ctypes mirror and checked by the tests)
   final val SIZEOF_COLUMN = 20; final val SIZEOF_EXPR = 20; final val SIZEOF_AGG = 8; final val SIZEOF_DESC = 104
   final val SIZEOF_LITERAL = 40
@@ -139,6 +142,9 @@ object GpuPlanSerializer {
       }
     }
 
+    /** the input of a two-input aggregate: a PAIR node over x and y (both DOUBLE) */
+    def pair(x: Expression, y: Expression): Int = node(Abi.PAIR, Abi.DOUBLE, add(x), add(y))
+
     def add(e0: Expression): Int = memo.getOrElseUpdate(e0, e0 match {
       case a: AttributeReference if aliases.contains(a.exprId) => add(aliases(a.exprId))   // ProjectExec inlined
       case a: AttributeReference => node(Abi.COL, typeOf(a), column(a))
@@ -217,6 +223,14 @@ object GpuPlanSerializer {
                 case _ => Abi.KURTOSIS
               }
               (fn, b.add(c))
+            case c @ (CovPopulation(_, _) | CovSample(_, _) | Corr(_, _)) =>
+              val Seq(x, y) = c.children
+              val fn = c match {
+                case _: CovPopulation => Abi.COVAR_POP
+                case _: CovSample => Abi.COVAR_SAMP
+                case _ => Abi.CORR
+              }
+              (fn, b.pair(x, y))
             case f => throw new Unsupported(s"aggregate function ${f.prettyName}")
           }
         }.toArray

@@ -44,16 +44,21 @@ class Op:
     ADD, SUB, MUL, DIV, NEG, CAST = 10, 11, 12, 13, 14, 15
     EQ, NE, LT, LE, GT, GE = 20, 21, 22, 23, 24, 25
     AND, OR, NOT, ISNULL, ISNOTNULL, IN, STARTSWITH = 30, 31, 32, 33, 34, 35, 36
+    PAIR = 37   # (x, y) input of COVAR_POP / COVAR_SAMP / CORR, both DOUBLE; nowhere else
 
 
 class AggFn:
     COUNT_STAR, COUNT, SUM, AVG, MIN, MAX = 1, 2, 3, 4, 5, 6
     # moment aggregates (Spark 2.1.1 CentralMomentAgg) over a DOUBLE input; stddev / variance are the SAMP forms
     STDDEV_POP, STDDEV_SAMP, VAR_POP, VAR_SAMP, SKEWNESS, KURTOSIS = 7, 8, 9, 10, 11, 12
+    # two-input aggregates (Spark 2.1.1 Covariance / Corr) over an Op.PAIR node of two DOUBLE inputs
+    COVAR_POP, COVAR_SAMP, CORR = 13, 14, 15
 
 
 # partial buffers of a moment aggregate, all non-nullable DOUBLE: [n, avg, m2] + [m3] (SKEWNESS) + [m3, m4] (KURTOSIS)
 MOMENT_BUFFERS = {AggFn.STDDEV_POP: 3, AggFn.STDDEV_SAMP: 3, AggFn.VAR_POP: 3, AggFn.VAR_SAMP: 3, AggFn.SKEWNESS: 4, AggFn.KURTOSIS: 5}
+# ... and of a two-input aggregate: [n, xAvg, yAvg, ck] + [xMk, yMk] (CORR)
+PAIR_BUFFERS = {AggFn.COVAR_POP: 4, AggFn.COVAR_SAMP: 4, AggFn.CORR: 6}
 
 
 class sd_column(C.Structure):
@@ -391,6 +396,8 @@ class PlanDesc:
                 out += [st if isinstance(st, tuple) else SqlType.DOUBLE, SqlType.LONG]
             elif fn in MOMENT_BUFFERS:
                 out += [SqlType.DOUBLE] * MOMENT_BUFFERS[fn]
+            elif fn in PAIR_BUFFERS:
+                out += [SqlType.DOUBLE] * PAIR_BUFFERS[fn]
             else:
                 out.append(self._ftype(e))
         return out
@@ -408,7 +415,7 @@ class PlanDesc:
                     out.append((SqlType.DECIMAL, min(38, p + 4), min(38, s + 4)))
                 else:
                     out.append(SqlType.DOUBLE)
-            elif fn in MOMENT_BUFFERS:
+            elif fn in MOMENT_BUFFERS or fn in PAIR_BUFFERS:
                 out.append(SqlType.DOUBLE)
             else:
                 out.append(self._ftype(e))

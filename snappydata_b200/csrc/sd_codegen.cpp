@@ -40,7 +40,7 @@ std::vector<int> partial_field_types(const PlanSpec& p) {
   std::vector<int> t;
   for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
   for (auto& m : p.agg_map) {
-    if (is_moment(m.fn)) { t.insert(t.end(), (size_t)agg_buffer_fields(m.fn), SD_DOUBLE); continue; }
+    if (is_moment(m.fn) || is_pair_agg(m.fn)) { t.insert(t.end(), (size_t)agg_buffer_fields(m.fn), SD_DOUBLE); continue; }
     t.push_back(field_type(m.buf_type, m.buf_ps)); if (m.fn == SD_AGG_AVG) t.push_back(SD_LONG);
   }
   return t;
@@ -98,7 +98,7 @@ static const char* opname(int op) {
     case SD_OP_EQ: return "eq"; case SD_OP_NE: return "ne"; case SD_OP_LT: return "lt"; case SD_OP_LE: return "le";
     case SD_OP_GT: return "gt"; case SD_OP_GE: return "ge"; case SD_OP_AND: return "and"; case SD_OP_OR: return "or";
     case SD_OP_NOT: return "not"; case SD_OP_ISNULL: return "isnull"; case SD_OP_ISNOTNULL: return "isnotnull";
-    case SD_OP_IN: return "in"; case SD_OP_STARTSWITH: return "startswith";
+    case SD_OP_IN: return "in"; case SD_OP_STARTSWITH: return "startswith"; case SD_OP_PAIR: return "pair";
   }
   return "?";
 }
@@ -249,6 +249,22 @@ struct Gen {
     for (auto& a : p.aggs) if (a.expr != -1 && !chk(a.expr)) return fail(SD_ERR_INVALID, "aggregate input out of range");
     for (int k : p.proj) if (!chk(k)) return fail(SD_ERR_INVALID, "projection expression out of range");
     if ((int)p.keys.size() > MAX_HASH_KEYS) return fail(SD_ERR_UNSUPPORTED, "more than 32 grouping keys");
+    // SD_OP_PAIR: two DOUBLE inputs of COVAR_POP / COVAR_SAMP / CORR, and nothing else
+    auto is_pair = [&](int n) { return p.exprs[n].op == SD_OP_PAIR; };
+    for (int i = 0; i < ne; i++) {
+      const sd_expr& e = p.exprs[i];
+      if (e.op == SD_OP_PAIR && (e.type != SD_DOUBLE || p.exprs[e.a].type != SD_DOUBLE || p.exprs[e.b].type != SD_DOUBLE))
+        return fail(SD_ERR_INVALID, "a PAIR node and both its inputs must be DOUBLE (cast them)");
+      if (e.op != SD_OP_COL && e.op != SD_OP_LIT && (is_pair(e.a) || (!is_unary(e.op) && is_pair(e.b))))
+        return fail(SD_ERR_INVALID, "a PAIR node is only the input of COVAR_POP / COVAR_SAMP / CORR, not of another operator");
+    }
+    if (p.filter >= 0 && is_pair(p.filter)) return fail(SD_ERR_INVALID, "a PAIR node cannot be a filter");
+    for (int k : p.keys) if (is_pair(k)) return fail(SD_ERR_INVALID, "a PAIR node cannot be a grouping key");
+    for (int k : p.proj) if (is_pair(k)) return fail(SD_ERR_INVALID, "a PAIR node cannot be projected or assigned");
+    for (auto& a : p.aggs) {
+      if (is_pair_agg(a.fn) && (a.expr < 0 || !is_pair(a.expr))) return fail(SD_ERR_INVALID, "COVAR_POP / COVAR_SAMP / CORR need a PAIR node input");
+      if (!is_pair_agg(a.fn) && a.expr >= 0 && is_pair(a.expr)) return fail(SD_ERR_INVALID, "a PAIR node is only the input of COVAR_POP / COVAR_SAMP / CORR");
+    }
     return 0;
   }
 
@@ -306,9 +322,10 @@ struct Gen {
     for (auto& a : p.aggs) {
       AggMap m;
       memset(&m, 0, sizeof(m));
-      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1; m.shift = -1;
+      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1; m.shift = -1; m.shift_y = -1;
       for (int& l : m.limb_slot) l = -1;
       for (int& s : m.pow_slot) s = -1;
+      for (int& s : m.pair_slot) s = -1;
       const int it = a.expr >= 0 ? p.exprs[a.expr].type : SD_LONG;
       const int in_null = a.expr >= 0 ? static_nullable(a.expr) : 0;
       m.in_type = it;
@@ -327,6 +344,33 @@ struct Gen {
         ShiftSpec* sh = &p.shifts[(size_t)m.shift];
         for (int j = 0; j < order; j++) sh->pow_slot[j] = m.pow_slot[j];
         sh->order = std::max(sh->order, order);
+        p.agg_map.push_back(m);
+        continue;
+      }
+      if (is_pair_agg(a.fn)) {
+        // n = the count of rows with x and y non-null; S_x, S_y, S_xy (+ CORR's S_xx, S_yy) around the group's (Kx, Ky)
+        const bool corr = a.fn == SD_AGG_CORR;
+        m.buf_type = SD_DOUBLE;
+        m.value_slot2 = -1;
+        m.count_slot = count_slot_for(a.expr);   // the PAIR node is NULL when x or y is
+        for (int j = 0; j < (corr ? 5 : 3); j++) m.pair_slot[j] = add_slot(SLOT_ADD_F64, a.expr, GATE_PAIR_X + j);
+        m.value_slot = m.pair_slot[2];
+        int q = -1;
+        for (size_t i = 0; i < p.pairs.size(); i++) if (p.pairs[i].xy_slot == m.pair_slot[2]) q = (int)i;   // same PAIR input
+        if (q < 0) {
+          p.shifts.push_back(ShiftSpec{1, {m.pair_slot[0], -1, -1, -1}});
+          p.shifts.push_back(ShiftSpec{1, {m.pair_slot[1], -1, -1, -1}});
+          p.pairs.push_back(PairSpec{(int)p.shifts.size() - 2, (int)p.shifts.size() - 1, m.pair_slot[2]});
+          q = (int)p.pairs.size() - 1;
+        }
+        m.shift = p.pairs[(size_t)q].shift_x;
+        m.shift_y = p.pairs[(size_t)q].shift_y;
+        if (corr) {   // the squares are the order-2 sums of the pair's x and y shifts
+          ShiftSpec &sx = p.shifts[(size_t)m.shift], &sy = p.shifts[(size_t)m.shift_y];
+          sx.order = sy.order = 2;
+          sx.pow_slot[1] = m.pair_slot[3];
+          sy.pow_slot[1] = m.pair_slot[4];
+        }
         p.agg_map.push_back(m);
         continue;
       }
@@ -621,6 +665,9 @@ struct Gen {
         o << "    const int t" << N << " = " << NL(e.a) << (e.op == SD_OP_ISNULL ? " ? 1 : 0;\n" : " ? 0 : 1;\n");
         finish_bool();
         return 0;
+      case SD_OP_PAIR:   // x as its value; the slots read y from child b (GATE_PAIR_Y)
+        o << "    const double v" << N << " = " << V(e.a) << "; const bool n" << N << " = " << NL(e.a) << " || " << NL(e.b) << ";\n";
+        return 0;
     }
     return fail(SD_ERR_INVALID, "unknown expression operator");
   }
@@ -733,6 +780,9 @@ struct Gen {
       else if (x.gate == GATE_VALUE_LO32) slt << NL << " ? 0ull : ((uint64_t)(int64_t)" << V << " & 0xffffffffull);\n";
       else if (x.gate == GATE_POW1) slt << NL << " ? sd::SHIFT_EMPTY : sd::shift_cand((double)" << V << ");\n";
       else if (x.gate >= GATE_POW2 && x.gate <= GATE_POW4) slt << "0ull;\n";
+      else if (x.gate == GATE_PAIR_X) slt << NL << " ? sd::SHIFT_EMPTY : sd::shift_cand(" << V << ");\n";
+      else if (x.gate == GATE_PAIR_Y) slt << NL << " ? sd::SHIFT_EMPTY : sd::shift_cand(v" << p.exprs[x.node].b << ");\n";
+      else if (x.gate >= GATE_PAIR_XY && x.gate <= GATE_PAIR_YY) slt << "0ull;\n";
       else {
         const bool f = x.op == SLOT_ADD_F64 || x.op == SLOT_MIN_F64 || x.op == SLOT_MAX_F64;
         char ident[32];
@@ -798,6 +848,16 @@ struct Gen {
       o << "  __host__ __device__ static constexpr int pow_slot(int i, int j) { return ";
       for (int i = 0; i < nsh; i++)
         for (int j = 1; j <= p.shifts[i].order; j++) o << "(i == " << i << " && j == " << j << ") ? " << p.shifts[i].pow_slot[j - 1] << " : ";
+      o << "0; }\n";
+    }
+    if (!p.pairs.empty()) {   // two-input aggregates: S_xy of shifts (x, y) (sd_kernels.cuh apply_shifts)
+      const int np = (int)p.pairs.size();
+      o << "  static constexpr int NPAIR = " << np << ";\n";
+      o << "  __host__ __device__ static constexpr int pair_shift(int q, int v) { return ";
+      for (int q = 0; q < np; q++) o << "(q == " << q << ") ? (v ? " << p.pairs[q].shift_y << " : " << p.pairs[q].shift_x << ") : ";
+      o << "0; }\n";
+      o << "  __host__ __device__ static constexpr int pair_slot(int q) { return ";
+      for (int q = 0; q < np; q++) o << "q == " << q << " ? " << p.pairs[q].xy_slot << " : ";
       o << "0; }\n";
     }
     o << "  struct Row {\n";

@@ -30,9 +30,13 @@ struct TableSpec {
 // GATE_DECREF: the value is a wide DECIMAL column held by reference (address of its [len][bytes] record)
 // GATE_POW1..4: S_j = sum (x - K)^j of a moment aggregate's input (the row leaves its candidate K, x, in S_1;
 // sd_kernels.cuh apply_shifts fills them all once the group's K is known)
+// GATE_PAIR_X / GATE_PAIR_Y: S_x = sum (x - Kx), S_y = sum (y - Ky) of a two-input aggregate's SD_OP_PAIR node (the row leaves
+// its candidate Kx / Ky there, SHIFT_EMPTY when x or y is NULL); GATE_PAIR_XY: S_xy = sum (x - Kx)(y - Ky); GATE_PAIR_XX /
+// GATE_PAIR_YY: CORR's sum (x - Kx)^2 / sum (y - Ky)^2.  apply_shifts fills them like the moment sums
 enum SlotGate { GATE_VALUE = 0, GATE_NONNULL_COUNT = 1, GATE_ONE = 2, GATE_VALUE_HI32 = 3, GATE_VALUE_LO32 = 4, GATE_STRREF = 5,
                 GATE_LIMB0 = 6, GATE_LIMB1 = 7, GATE_LIMB2 = 8, GATE_LIMB3 = 9, GATE_DECREF = 10,
-                GATE_POW1 = 11, GATE_POW2 = 12, GATE_POW3 = 13, GATE_POW4 = 14 };
+                GATE_POW1 = 11, GATE_POW2 = 12, GATE_POW3 = 13, GATE_POW4 = 14,
+                GATE_PAIR_X = 15, GATE_PAIR_Y = 16, GATE_PAIR_XY = 17, GATE_PAIR_XX = 18, GATE_PAIR_YY = 19 };
 
 struct SlotSpec {
   int op;     // SLOT_*
@@ -55,19 +59,33 @@ struct AggMap {
   int limb_slot[4]; // SUM/AVG of a wide DECIMAL: the slots of limbs 0..3 (value_slot = limb 3, value_slot2 = -1); else -1
   int shift;        // moment aggregate: index of its input's shift in PlanSpec.shifts (count_slot = n, value_slot = S_1); else -1
   int pow_slot[4];  // moment aggregate: S_1..S_order; else -1
+  int shift_y;      // two-input aggregate: index of its y shift (`shift` is the x shift; count_slot = n, value_slot = S_xy); else -1
+  int pair_slot[5]; // two-input aggregate: S_x, S_y, S_xy, S_xx, S_yy (the last two CORR only); else -1
 };
 
 // a moment aggregate (Spark 2.1.1 CentralMomentAgg): STDDEV_* / VAR_* (order 2), SKEWNESS (3), KURTOSIS (4)
 inline bool is_moment(int fn) { return fn >= SD_AGG_STDDEV_POP && fn <= SD_AGG_KURTOSIS; }
 inline int moment_order(int fn) { return fn == SD_AGG_KURTOSIS ? 4 : fn == SD_AGG_SKEWNESS ? 3 : 2; }
-// partial-row buffer fields of an aggregate: AVG [sum, count]; moments [n, avg, m2, (m3, (m4))]; others one
-inline int agg_buffer_fields(int fn) { return fn == SD_AGG_AVG ? 2 : is_moment(fn) ? 1 + moment_order(fn) : 1; }
+// a two-input aggregate (Spark 2.1.1 Covariance / Corr) over an SD_OP_PAIR node
+inline bool is_pair_agg(int fn) { return fn >= SD_AGG_COVAR_POP && fn <= SD_AGG_CORR; }
+// partial-row buffer fields of an aggregate: AVG [sum, count]; moments [n, avg, m2, (m3, (m4))]; COVAR_* [n, xAvg, yAvg, ck];
+// CORR [n, xAvg, yAvg, ck, xMk, yMk]; others one
+inline int agg_buffer_fields(int fn) {
+  return fn == SD_AGG_AVG ? 2 : is_moment(fn) ? 1 + moment_order(fn) : fn == SD_AGG_CORR ? 6 : is_pair_agg(fn) ? 4 : 1;
+}
 
 // one shift K of a plan's moment sums (its K words are not slots, sd_device.h SHIFT_EMPTY): every moment aggregate over the
 // same input shares it and its S_j slots
 struct ShiftSpec {
   int order;        // highest power summed
   int pow_slot[4];  // S_1..S_order
+};
+
+// the cross term of a two-input aggregate's shifts: S_xy = sum (x - Kx)(y - Ky).  Its x and y shifts are ordinary ShiftSpecs
+// (order 1, or 2 when CORR needs the squares); COVAR_* and CORR over the same PAIR share them, a moment aggregate over x does not
+struct PairSpec {
+  int shift_x, shift_y;
+  int xy_slot;
 };
 
 // field type codes used for rows on the host: sd_type in the low byte, DECIMAL precision/scale above it
@@ -94,6 +112,7 @@ struct PlanSpec {
   std::vector<SlotSpec> slots;
   std::vector<AggMap> agg_map;
   std::vector<ShiftSpec> shifts;     // moment aggregates' shifts: K words [group][shift] beside the slots
+  std::vector<PairSpec> pairs;       // two-input aggregates' cross terms over two of those shifts
   int rows_slot = -1;                // COUNT(*)-like slot that tells which groups exist
   int mode = 0;                      // MODE_NOKEY | MODE_GROUPS | MODE_HASH | MODE_PROJECT | MODE_MUTATE
   int rpt = 4;                       // rows per thread per tile (2, 4, 8)

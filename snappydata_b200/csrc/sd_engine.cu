@@ -1249,6 +1249,31 @@ void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, const uint64_t* k
       for (int j = 0; j <= order; j++) { HVal f; f.d = b[j]; vals.push_back(f); }
       continue;
     }
+    if (is_pair_agg(m.fn)) {   // Spark's buffers [n, xAvg, yAvg, ck, (xMk, yMk)] from n, S_x, S_y, S_xy (, S_xx, S_yy)
+      const bool corr = m.fn == SD_AGG_CORR;
+      double b[6] = {0, 0, 0, 0, 0, 0};
+      if (cnt > 0) {
+        const double n = (double)cnt, Kx = u2f_host(kw[m.shift]), Ky = u2f_host(kw[m.shift_y]);
+        const double Sx = u2f_host(sv[m.pair_slot[0]]), Sy = u2f_host(sv[m.pair_slot[1]]), Sxy = u2f_host(sv[m.pair_slot[2]]);
+        const double dx = Sx / n, dy = Sy / n;
+        b[0] = n;
+        if (!std::isfinite(Kx) || !std::isfinite(Ky) || !std::isfinite(Sx) || !std::isfinite(Sy)) {
+          // a counted row had a NaN or +-Inf x or y (its shifted value, or the group's K, is not finite): NaN, not the +-Inf
+          // some shifted sums would give
+          for (int j = 1; j < 6; j++) b[j] = NAN;
+        } else {
+          b[1] = Kx + dx;
+          b[2] = Ky + dy;
+          b[3] = Sxy - n * dx * dy;
+          if (corr) {
+            b[4] = std::max(0.0, u2f_host(sv[m.pair_slot[3]]) - n * dx * dx);   // >= 0 despite rounding (S_x, S_y are finite here)
+            b[5] = std::max(0.0, u2f_host(sv[m.pair_slot[4]]) - n * dy * dy);
+          }
+        }
+      }
+      for (int j = 0; j < (corr ? 6 : 4); j++) { HVal f; f.d = b[j]; vals.push_back(f); }
+      continue;
+    }
     if (m.value_slot2 >= 0) {   // DECIMAL SUM / AVG: high and low halves summed separately (sd_codegen.cpp build_slots)
       v.w = (i128)(int64_t)sv[m.value_slot] * ((i128)1 << 32) + (i128)(int64_t)sv[m.value_slot2];
       v.i = (int64_t)v.w;
@@ -2175,7 +2200,7 @@ void sd_plan_destroy(sd_plan* p) {
 int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32_t* slot_is_f64) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_partials_layout: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
-  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: moment sums of different GPUs are shifted differently and do not add");
+  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: shifted sums (moments, covariance) of different GPUs do not add");
   const int ns = (int)p->spec.slots.size();
   if (ngroups) *ngroups = p->ngroups;
   if (nslots) *nslots = ns;
@@ -2186,7 +2211,7 @@ int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_export_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_out) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
-  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: moment sums of different GPUs are shifted differently and do not add");
+  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: shifted sums (moments, covariance) of different GPUs do not add");
   SD_CUDA(cudaSetDevice(p->device));
   int rc = flush_pending(p);
   if (rc) return rc;
@@ -2200,7 +2225,7 @@ int sd_plan_import_partials(sd_plan* p, const void* dev_in, int64_t bytes) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_import_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_in) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
-  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: moment sums of different GPUs are shifted differently and do not add");
+  if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: shifted sums (moments, covariance) of different GPUs do not add");
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
   SD_CUDA(cudaSetDevice(p->device));
@@ -2347,6 +2372,32 @@ static void moment_merge(HVal* b, const HVal* in, int order) {
     b[4].d = b[4].d + in[4].d + dN * dN * dN * delta * n1 * n2 * (n1 * n1 - n1 * n2 + n2 * n2) + 6.0 * dN * dN * (n1 * n1 * m2b + n2 * n2 * m2a) +
              4.0 * dN * (n1 * m3b - n2 * m3a);
 }
+// Covariance / Corr (Spark 2.1.1) on the buffers [n, xAvg, yAvg, ck, (xMk, yMk)]: mergeExpressions ...
+static void pair_merge(HVal* b, const HVal* in, bool corr) {
+  const double n1 = b[0].d, n2 = in[0].d, n = n1 + n2;
+  const double dx = in[1].d - b[1].d, dxN = n == 0.0 ? 0.0 : dx / n;
+  const double dy = in[2].d - b[2].d, dyN = n == 0.0 ? 0.0 : dy / n;
+  b[0].d = n;
+  b[1].d = b[1].d + dxN * n2;
+  b[2].d = b[2].d + dyN * n2;
+  b[3].d = b[3].d + in[3].d + dx * dyN * n1 * n2;
+  if (corr) {
+    b[4].d = b[4].d + in[4].d + dx * dxN * n1 * n2;
+    b[5].d = b[5].d + in[5].d + dy * dyN * n1 * n2;
+  }
+}
+// ... and evaluateExpression: NULL without input
+static HVal pair_result(int fn, const HVal* b) {
+  HVal v;
+  const double n = b[0].d, ck = b[3].d;
+  if (n == 0.0) { v.isnull = true; return v; }
+  switch (fn) {
+    case SD_AGG_COVAR_POP: v.d = ck / n; break;
+    case SD_AGG_COVAR_SAMP: v.d = n == 1.0 ? NAN : ck / (n - 1.0); break;
+    default: v.d = n == 1.0 ? NAN : ck / std::sqrt(b[4].d * b[5].d); break;   // SD_AGG_CORR
+  }
+  return v;
+}
 // ... and evaluateExpression: NULL without input; stddev / variance are the SAMP forms
 static HVal moment_result(int fn, const HVal* b) {
   HVal v;
@@ -2416,6 +2467,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
         HVal& b = g->bufs[k];
         const HVal& in = f[nk + k];
         if (is_moment(m.fn)) { moment_merge(&b, &in, moment_order(m.fn)); k += agg_buffer_fields(m.fn); continue; }
+        if (is_pair_agg(m.fn)) { pair_merge(&b, &in, m.fn == SD_AGG_CORR); k += agg_buffer_fields(m.fn); continue; }
         switch (m.fn) {
           case SD_AGG_COUNT_STAR: case SD_AGG_COUNT: b.i += in.i; k++; break;
           case SD_AGG_SUM:
@@ -2463,6 +2515,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
       int k = 0;
       for (auto& m : sp.agg_map) {
         if (is_moment(m.fn)) { vals.push_back(moment_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
+        if (is_pair_agg(m.fn)) { vals.push_back(pair_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
         if (m.fn == SD_AGG_AVG) {   // Average.evaluateExpression: sum / count, NULL when count == 0
           HVal v;
           const int64_t cnt = g.bufs[k + 1].i;

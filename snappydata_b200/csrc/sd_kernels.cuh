@@ -239,6 +239,10 @@ __device__ __forceinline__ int64_t hash_find_or_insert(const HashTable& t, const
 // ((mean - K) / sigma)^order, not to (mean / sigma)^order as raw power sums would.
 template <class P, class = void> struct PlanShifts { static constexpr int N = 0; };
 template <class P> struct PlanShifts<P, decltype((void)P::NSHIFT)> { static constexpr int N = P::NSHIFT; };
+// COVAR_POP / COVAR_SAMP / CORR: NPAIR > 0 cross terms S_xy = sum (x - Kx)(y - Ky), each over two of the shifts above
+// (pair_shift(q, 0) = x, pair_shift(q, 1) = y; the squares CORR needs are those shifts' order-2 sums) into slot pair_slot(q)
+template <class P, class = void> struct PlanPairs { static constexpr int N = 0; };
+template <class P> struct PlanPairs<P, decltype((void)P::NPAIR)> { static constexpr int N = P::NPAIR; };
 
 __device__ __forceinline__ uint64_t shift_cand(double x) { return x != x ? 0x7ff8000000000000ull : f2u(x); }
 // the group's K in the word at p (beside the running result or the hash entry), claimed with `cand` while still SHIFT_EMPTY
@@ -254,17 +258,26 @@ __device__ __forceinline__ uint64_t shift_claim(uint64_t* p, uint64_t cand) {
 // kof(i, cand) -> the group's K of shift i
 template <class PLAN, class KOf>
 __device__ __forceinline__ void apply_shifts(uint64_t* sv, KOf&& kof) {
+  constexpr int NP = PlanPairs<PLAN>::N;
+  double dv[NP > 0 ? PLAN::NSHIFT : 1];   // x - K per shift (0 for a NULL input), kept for the cross terms
+  (void)dv;
 #pragma unroll
   for (int i = 0; i < PLAN::NSHIFT; i++) {
     const uint64_t cand = sv[PLAN::pow_slot(i, 1)];
+    if constexpr (NP > 0) dv[i] = 0.0;
     if (cand == SHIFT_EMPTY) { sv[PLAN::pow_slot(i, 1)] = 0ull; continue; }   // NULL input: its sums stay 0
     const double d = u2f(cand) - u2f(kof(i, cand));
+    if constexpr (NP > 0) dv[i] = d;
     double pw = d;
 #pragma unroll
     for (int j = 1; j <= 4; j++) {
       if (j <= PLAN::order(i)) sv[PLAN::pow_slot(i, j)] = f2u(pw);
       pw *= d;
     }
+  }
+  if constexpr (NP > 0) {
+#pragma unroll
+    for (int q = 0; q < NP; q++) sv[PLAN::pair_slot(q)] = f2u(dv[PLAN::pair_shift(q, 0)] * dv[PLAN::pair_shift(q, 1)]);
   }
 }
 

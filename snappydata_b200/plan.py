@@ -109,6 +109,11 @@ class PlanBuilder:
     def skewness(self, e: E): return self.agg(AggFn.SKEWNESS, e)
     def kurtosis(self, e: E): return self.agg(AggFn.KURTOSIS, e)
     stddev, variance = stddev_samp, var_samp
+    # two-input aggregates over a PAIR node of DOUBLE inputs (Spark casts them too): x.cast(SqlType.DOUBLE)
+    def pair(self, x: E, y: E) -> E: return E(self, Op.PAIR, SqlType.DOUBLE, x, y)
+    def covar_pop(self, x: E, y: E): return self.agg(AggFn.COVAR_POP, self.pair(x, y))
+    def covar_samp(self, x: E, y: E): return self.agg(AggFn.COVAR_SAMP, self.pair(x, y))
+    def corr(self, x: E, y: E): return self.agg(AggFn.CORR, self.pair(x, y))
     def project(self, *es: E): self._proj = list(es); return self
 
     # UPDATE / DELETE over a resident store (SD_PLAN_MUTATE; the WHERE clause is filter())
