@@ -81,8 +81,11 @@ typedef enum sd_op {
   SD_OP_ISNULL = 33, SD_OP_ISNOTNULL = 34,
   SD_OP_IN = 35,        /* a = expr, b = first literal slot, c = number of literals */
   SD_OP_STARTSWITH = 36, /* a = string expr, b = literal node                    */
-  SD_OP_PAIR = 37       /* a = x node, b = y node, both DOUBLE; type DOUBLE, NULL when either is NULL.  Only as the input
+  SD_OP_PAIR = 37,      /* a = x node, b = y node, both DOUBLE; type DOUBLE, NULL when either is NULL.  Only as the input
                            of a two-input aggregate (COVAR_POP / COVAR_SAMP / CORR); anywhere else SD_ERR_INVALID */
+  SD_OP_GROUPING_SET = 38, /* type SD_INT, a = one grouping-set mask.  Only as a member of a GROUPING_ID node's list */
+  SD_OP_GROUPING_ID = 39   /* type SD_INT, a = index of the first of b consecutive GROUPING_SET nodes; only as the LAST entry of
+                              sd_plan_desc.keys (GROUP BY ... WITH ROLLUP / WITH CUBE / GROUPING SETS, see below) */
 } sd_op;
 
 typedef struct sd_expr {
@@ -142,7 +145,20 @@ typedef struct sd_expr {
  * ck/sqrt(xMk*yMk).  The device sums (x - Kx), (y - Ky), (x - Kx)(y - Ky) (and for CORR the squares) around one shift pair
  * (Kx, Ky) per group and input pair.  A group in which a counted row has a NaN or +-Inf x or y gets NaN in every buffer but n,
  * so its results are NaN (Spark's row-order update gives +-Inf or NaN there, depending on where the row falls).  Plans with
- * these aggregates have no dense partials export either. */
+ * these aggregates have no dense partials export either.
+ * Grouping sets (Spark 2.1.1 Expand under the partial aggregate for GROUP BY ... WITH ROLLUP / WITH CUBE / GROUPING SETS; the
+ * analyzer rule ResolveGroupingAnalytics is restated from upstream Spark, the fork's source is not at hand).  The last key is an
+ * SD_OP_GROUPING_ID node; the n keys before it are the GROUP BY expressions.  Each GROUPING_SET mask follows SnappyParser's
+ * convention (core/SnappyParser.scala:564-571): bit (n-1-k) set <=> key k is absent from the set (NULL in its rows).  ROLLUP(k1..kn)
+ * = masks (1 << i) - 1 for i = 0..n, CUBE = 0 .. 2^n - 1.  Partial rows are UnsafeRow(k1..kn, gid, aggregate buffers) and final
+ * rows keys ++ gid ++ one value per aggregate, gid = the set's mask (INT, NOT NULL): a key absent from a set and a key NULL in the
+ * data are different groups.  Aggregate inputs read the original values in every set; no input rows, no output rows (not even
+ * for the () set).  sd_final_merge / sd_partial_merge treat gid as one more INT key.  The device scans once with the plain
+ * GROUP BY k1..kn kernel and rolls its groups up into every set.  SD_ERR_INVALID: a GROUPING_SET node that is not in a
+ * GROUPING_ID list; a GROUPING_ID node that is not the last key, or that is an operand, a filter, an aggregate input, a projection
+ * or a SET value; a mask with bits at or above n; b < 1.  SD_ERR_UNSUPPORTED: duplicate masks; n == 0 (no GROUP BY expression
+ * before the GROUPING_ID); n > 31; more than 4096 sets; more than 16 moment / covariance shifts (one per distinct moment input,
+ * two per distinct PAIR); a GROUPING_ID in an SD_PLAN_MUTATE or projection plan.  These plans have no dense partials export. */
 typedef enum sd_agg_fn {
   SD_AGG_COUNT_STAR = 1, SD_AGG_COUNT = 2, SD_AGG_SUM = 3, SD_AGG_AVG = 4, SD_AGG_MIN = 5, SD_AGG_MAX = 6,
   SD_AGG_STDDEV_POP = 7, SD_AGG_STDDEV_SAMP = 8, SD_AGG_VAR_POP = 9, SD_AGG_VAR_SAMP = 10, SD_AGG_SKEWNESS = 11,
@@ -472,6 +488,10 @@ enum { SDX_REPLAY_NONE = 0,
        SDX_REPLAY_HASH_GROW = 2,     /* the hash table grew: every launch of the execution re-runs                      */
        SDX_REPLAY_ROWS_GROW = 3 };   /* the projection / UPDATE / DELETE record buffer grew: every launch re-runs       */
 int sdx_plan_launch_log(sd_plan* p, int64_t* out, int32_t cap, int32_t* n);
+/* the roll-up of a grouping-sets plan's last execution (test / bench hook; the launch log and sd_plan_metrics cover the scan
+ * only): [0] roll-up device ms (CUDA events, re-runs included) [1] fine groups of the scan [2] coarse groups emitted
+ * [3] roll-up launches (a re-run after the roll-up table overflowed counts again).  All 0 for other plans. */
+int sdx_plan_rollup_info(sd_plan* p, double out[4]);
 /* expand n raw LZ4 blocks with the engine's device kernel (bench/test hook used by tools/lz4_bench.py): uploads the
  * blocks, places output i at a 16-byte boundary + dst_misalign, runs `reps` launches timed with CUDA events
  * (ms_per_launch = their mean) and copies output i to outs[i] when outs != NULL.  `dense` selects the kernel variant:

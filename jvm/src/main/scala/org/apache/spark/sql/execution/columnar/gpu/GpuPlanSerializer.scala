@@ -25,7 +25,7 @@ import org.apache.spark.sql.catalyst.expressions.aggregate._
 import org.apache.spark.sql.catalyst.expressions.codegen.{BufferHolder, UnsafeRowWriter}
 import org.apache.spark.sql.catalyst.util.DateTimeUtils
 import org.apache.spark.sql.collection.SharedUtils
-import org.apache.spark.sql.execution.{FilterExec, ProjectExec, SparkPlan}
+import org.apache.spark.sql.execution.{ExpandExec, FilterExec, ProjectExec, SparkPlan}
 import org.apache.spark.sql.execution.aggregate.SnappyHashAggregateExec
 import org.apache.spark.sql.execution.columnar.{ColumnBatchIterator, ColumnTableScan}
 import org.apache.spark.sql.execution.columnar.impl.{ColumnDelta, ColumnFormatEntry}
@@ -49,6 +49,8 @@ private[gpu] object Abi {
   final val AND = 30; final val OR = 31; final val NOT = 32; final val ISNULL = 33; final val ISNOTNULL = 34
   final val IN = 35; final val STARTSWITH = 36
   final val PAIR = 37   // (x, y) input of COVAR_POP / COVAR_SAMP / CORR
+  final val GROUPING_SET = 38   // INT, a = one grouping-set mask; only in a GROUPING_ID node's list
+  final val GROUPING_ID = 39    // INT, a = first of b GROUPING_SET nodes; only as the last grouping key
   // sd_agg_fn
   final val COUNT_STAR = 1; final val COUNT = 2; final val SUM = 3; final val AVG = 4; final val MIN = 5; final val MAX = 6
   // CentralMomentAgg: the child is DOUBLE (ImplicitCastInputTypes puts a Cast in front of any other numeric input)
@@ -142,6 +144,13 @@ object GpuPlanSerializer {
       }
     }
 
+    /** spark_grouping_id of GROUP BY ... WITH ROLLUP / CUBE / GROUPING SETS: the set nodes, then the GROUPING_ID node */
+    def groupingId(masks: Seq[Int]): Int = {
+      val first = exprs.length
+      masks.foreach(m => node(Abi.GROUPING_SET, Abi.INT, m))
+      node(Abi.GROUPING_ID, Abi.INT, first, masks.length)
+    }
+
     /** the input of a two-input aggregate: a PAIR node over x and y (both DOUBLE) */
     def pair(x: Expression, y: Expression): Int = node(Abi.PAIR, Abi.DOUBLE, add(x), add(y))
 
@@ -184,6 +193,42 @@ object GpuPlanSerializer {
     })
   }
 
+  /** GROUP BY ... WITH ROLLUP / WITH CUBE / GROUPING SETS as upstream Spark 2.1.1's ResolveGroupingAnalytics plans it (restated;
+    * the fork's analyzer source is not at hand): ExpandExec(projections, output, ProjectExec(c ++ groupByAliases, ...)) under
+    * the partial aggregate, where every projection is  c ++ (per GROUP BY key: its attribute | null literal) ++ Literal(mask)
+    * and output = c ++ the keys' new instances ++ gid, the aggregate grouping by those n + 1 attributes.  The mask of a
+    * projection must be the one its null literals spell in SnappyParser's convention (bit n-1-k set <=> key k absent,
+    * core/SnappyParser.scala:564-571).  Returns (the n key attributes of Expand's child, the masks); None for any other Expand --
+    * e.g. RewriteDistinctAggregates', whose projections null aggregate inputs, not keys. */
+  private def groupingSets(agg: SnappyHashAggregateExec, e: ExpandExec): Option[(Seq[Attribute], Seq[Int])] = {
+    val n = agg.groupingExpressions.length - 1
+    val c = e.output.length - n - 1
+    if (n < 1 || c < 0 || e.child.output.length != c + n || e.projections.isEmpty) return None
+    val grouped = agg.groupingExpressions.map {
+      case a: Attribute => Some(a.exprId)
+      case _ => None
+    }
+    if (grouped != e.output.drop(c).map(a => Some(a.exprId))) return None
+    if (e.output.last.dataType != IntegerType || e.output.last.nullable) return None
+    val prefix = e.child.output.take(c).map(_.exprId)
+    val keys = e.child.output.drop(c)
+    val masks = e.projections.map { p =>
+      if (p.length != c + n + 1) return None
+      if (p.take(c).map { case a: Attribute => Some(a.exprId); case _ => None } != prefix.map(Some(_))) return None
+      var mask = 0
+      for (i <- 0 until n) p(c + i) match {
+        case a: Attribute if a.exprId == keys(i).exprId =>
+        case Literal(null, _) => mask |= 1 << (n - 1 - i)
+        case _ => return None
+      }
+      p(c + n) match {
+        case Literal(m: Int, IntegerType) if m == mask => mask
+        case _ => return None
+      }
+    }
+    if (masks.distinct.length != masks.length) None else Some((keys, masks))   // duplicate sets: refused by the library too
+  }
+
   /** Some(desc) iff the fragment is SnappyHashAggregateExec(Partial) over [Project] [Filter] ColumnTableScan
     * (core/.../aggregate/SnappyHashAggregateExec.scala:72-80; planned at StoreDataSourceStrategy.scala:128-130,236-240)
     * with expressions the C ABI expresses and a plan the library accepts; anything else stays on the stock operators.
@@ -199,11 +244,23 @@ object GpuPlanSerializer {
       case _ => None
     }
     if (agg.hasDistinct || !agg.aggregateExpressions.forall(a => a.mode == Partial && !a.isDistinct)) return None
-    unwrap(agg.child, Nil, Map.empty).flatMap { case (scan, filters, aliases) =>
+    // ROLLUP / CUBE / GROUPING SETS: Expand directly under the aggregate, in ResolveGroupingAnalytics' shape only
+    val (below, sets) = agg.child match {
+      case e: ExpandExec => groupingSets(agg, e) match {
+        case Some(s) => (e.child, Some(s))
+        case None => return None
+      }
+      case other => (other, None)
+    }
+    unwrap(below, Nil, Map.empty).flatMap { case (scan, filters, aliases) =>
       try {
         val b = new Builder(scan, aliases)
         val filter = if (filters.isEmpty) -1 else b.add(filters.reduce(And))
-        val keys = agg.groupingExpressions.map(b.add(_)).toArray
+        // grouping sets: the GROUP BY keys (Expand's child projects them as aliases); spark_grouping_id follows below
+        val groupKeys = sets match {
+          case Some((attrs, _)) => attrs.map(b.add(_)).toArray
+          case None => agg.groupingExpressions.map(b.add(_)).toArray
+        }
         val aggs = agg.aggregateExpressions.map { ae =>
           ae.aggregateFunction match {
             case Count(Seq(l)) if l.foldable && l.eval(null) != null => (Abi.COUNT_STAR, -1)   // count(*) == count(1)
@@ -234,6 +291,8 @@ object GpuPlanSerializer {
             case f => throw new Unsupported(s"aggregate function ${f.prettyName}")
           }
         }.toArray
+        // the set nodes come last, so that the scan's generated source is the plain GROUP BY's
+        val keys = sets.fold(groupKeys)(s => groupKeys :+ b.groupingId(s._2))
         // make sure every scan column the kernel must read exists even when only count(*) is asked for
         val addr = write(b, filter, keys, aggs)
         // the library validates the plan (types, casts, limits) and compiles / finds its kernel: probe it once here

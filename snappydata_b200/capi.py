@@ -45,6 +45,8 @@ class Op:
     EQ, NE, LT, LE, GT, GE = 20, 21, 22, 23, 24, 25
     AND, OR, NOT, ISNULL, ISNOTNULL, IN, STARTSWITH = 30, 31, 32, 33, 34, 35, 36
     PAIR = 37   # (x, y) input of COVAR_POP / COVAR_SAMP / CORR, both DOUBLE; nowhere else
+    GROUPING_SET = 38   # INT, a = one grouping-set mask; only in a GROUPING_ID node's list
+    GROUPING_ID = 39    # INT, a = first of b GROUPING_SET nodes; only as the last grouping key
 
 
 class AggFn:
@@ -289,6 +291,8 @@ def product_api() -> Api:
         L.sdx_store_get_delta.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
         L.sdx_store_get_deletes.restype = C.c_int
         L.sdx_store_get_deletes.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
+        L.sdx_plan_rollup_info.restype = C.c_int
+        L.sdx_plan_rollup_info.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         L.sdx_last_mutation_timing.restype = C.c_int
         L.sdx_last_mutation_timing.argtypes = [C.POINTER(C.c_double)]
         L.sd_store_compact.restype = C.c_int
@@ -600,6 +604,12 @@ class Plan:
                         "paths": dict(zip(BATCH_PATHS, w[8:12])), "replay": LAUNCH_REPLAYS[w[12]],
                         "nbatches": w[13], "chunks": w[14], "streamed_bytes": w[15]})
         return out
+
+    def rollup_info(self) -> Dict[str, float]:
+        """The grouping-sets roll-up of the last execution (sdx_plan_rollup_info)."""
+        out = (C.c_double * 4)()
+        self.api.check(self.api.lib.sdx_plan_rollup_info(self.h, out))
+        return {"ms": out[0], "fine": int(out[1]), "coarse": int(out[2]), "launches": int(out[3])}
 
     def set_option(self, option: int, value: int):
         self.api.check(self.api.plan_set_option(self.h, option, value))

@@ -39,6 +39,7 @@ static const char* col_ctype(const sd_column& c);
 std::vector<int> partial_field_types(const PlanSpec& p) {
   std::vector<int> t;
   for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
+  if (p.gid_node >= 0) t.push_back(SD_INT);   // spark_grouping_id
   for (auto& m : p.agg_map) {
     if (is_moment(m.fn) || is_pair_agg(m.fn)) { t.insert(t.end(), (size_t)agg_buffer_fields(m.fn), SD_DOUBLE); continue; }
     t.push_back(field_type(m.buf_type, m.buf_ps)); if (m.fn == SD_AGG_AVG) t.push_back(SD_LONG);
@@ -48,6 +49,7 @@ std::vector<int> partial_field_types(const PlanSpec& p) {
 std::vector<int> final_field_types(const PlanSpec& p) {
   std::vector<int> t;
   for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
+  if (p.gid_node >= 0) t.push_back(SD_INT);
   for (auto& m : p.agg_map) {
     if (m.fn == SD_AGG_AVG) {
       if (m.buf_type == SD_DECIMAL) {   // Average.resultType: DecimalType.bounded(p + 4, s + 4)
@@ -106,6 +108,7 @@ static bool is_unary(int op) {
   return op == SD_OP_NEG || op == SD_OP_CAST || op == SD_OP_NOT || op == SD_OP_ISNULL || op == SD_OP_ISNOTNULL || op == SD_OP_IN;
 }
 static bool is_cmp(int op) { return op >= SD_OP_EQ && op <= SD_OP_GE; }
+static bool is_grouping_node(int op) { return op == SD_OP_GROUPING_SET || op == SD_OP_GROUPING_ID; }
 
 sd_plan_desc PlanSpec::desc_view() const {
   sd_plan_desc d;
@@ -114,7 +117,7 @@ sd_plan_desc PlanSpec::desc_view() const {
   d.ncols = (int)cols.size(); d.cols = cols.data();
   d.nexprs = (int)exprs.size(); d.exprs = exprs.data();
   d.filter = filter;
-  d.nkeys = (int)keys.size(); d.keys = keys.data();
+  d.nkeys = (int)desc_keys.size(); d.keys = desc_keys.data();
   d.naggs = (int)aggs.size(); d.aggs = aggs.data();
   d.nproj = (int)proj.size(); d.proj = proj.data();
   d.nliterals = (int)literal_types.size(); d.literal_types = literal_types.data();
@@ -199,6 +202,61 @@ struct Gen {
 
   int fail(int code, const std::string& m) { err = m; return code; }
 
+  // GROUP BY ... WITH ROLLUP / CUBE / GROUPING SETS: a GROUPING_ID node as the last key lists the sets' masks; it is taken out of
+  // `keys` so that everything generated from here on is the plain GROUP BY over the keys before it
+  int grouping_sets() {
+    const int ne = (int)p.exprs.size(), nk = (int)p.keys.size();
+    std::vector<char> member(ne, 0);
+    for (int i = 0; i < ne; i++) {
+      const sd_expr& e = p.exprs[i];
+      if (e.op == SD_OP_GROUPING_SET && e.type != SD_INT) return fail(SD_ERR_INVALID, "a GROUPING_SET node has type INT");
+      if (e.op != SD_OP_GROUPING_ID) continue;
+      if (e.type != SD_INT) return fail(SD_ERR_INVALID, "a GROUPING_ID node has type INT");
+      if (e.b < 1) return fail(SD_ERR_INVALID, "a GROUPING_ID node lists at least one grouping set");
+      if (e.a < 0 || e.a + (int64_t)e.b > i) return fail(SD_ERR_INVALID, "a GROUPING_ID node's sets must precede it");
+      for (int j = e.a; j < e.a + e.b; j++) {
+        if (p.exprs[j].op != SD_OP_GROUPING_SET) return fail(SD_ERR_INVALID, "a GROUPING_ID node lists consecutive GROUPING_SET nodes");
+        member[j] = 1;
+      }
+    }
+    for (int i = 0; i < ne; i++) {
+      const sd_expr& e = p.exprs[i];
+      if (e.op == SD_OP_GROUPING_SET && !member[i]) return fail(SD_ERR_INVALID, "a GROUPING_SET node outside a GROUPING_ID list");
+      if (e.op == SD_OP_COL || e.op == SD_OP_LIT || is_grouping_node(e.op)) continue;
+      const bool bin = !is_unary(e.op);
+      auto bad = [&](int c) { return c >= 0 && c < ne && is_grouping_node(p.exprs[c].op); };
+      if (bad(e.a) || (bin && bad(e.b))) return fail(SD_ERR_INVALID, "a GROUPING_SET / GROUPING_ID node is not an operand");
+    }
+    auto is_gid = [&](int n) { return n >= 0 && n < ne && is_grouping_node(p.exprs[n].op); };
+    if (is_gid(p.filter)) return fail(SD_ERR_INVALID, "a GROUPING_ID node cannot be a filter");
+    for (auto& a : p.aggs) if (is_gid(a.expr)) return fail(SD_ERR_INVALID, "a GROUPING_ID node cannot be an aggregate input");
+    for (int k : p.proj) if (is_gid(k)) return fail(SD_ERR_INVALID, "a GROUPING_ID node cannot be projected or assigned");
+    for (int k = 0; k < nk; k++) {
+      if (!is_gid(p.keys[k])) continue;
+      if (p.exprs[p.keys[k]].op != SD_OP_GROUPING_ID || k != nk - 1) return fail(SD_ERR_INVALID, "a GROUPING_ID node is only the last grouping key");
+    }
+    const int last = nk > 0 && is_gid(p.keys[nk - 1]) ? p.keys[nk - 1] : -1;
+    for (int i = 0; i < ne; i++)
+      if (p.exprs[i].op == SD_OP_GROUPING_ID && i != last) return fail(SD_ERR_INVALID, "a GROUPING_ID node is only the last grouping key");
+    if (last < 0) return 0;
+    if (p.flags & SD_PLAN_MUTATE) return fail(SD_ERR_UNSUPPORTED, "GROUPING_ID in an UPDATE / DELETE plan");
+    if (p.aggs.empty() && nk == 1) return fail(SD_ERR_UNSUPPORTED, "GROUPING_ID in a projection plan");
+    const sd_expr& g = p.exprs[p.keys[nk - 1]];
+    const int n = nk - 1;
+    if (n == 0) return fail(SD_ERR_UNSUPPORTED, "grouping sets without GROUP BY expressions");
+    if (n > 31) return fail(SD_ERR_UNSUPPORTED, "grouping sets over more than 31 GROUP BY expressions (spark_grouping_id is an INT)");
+    if (g.b > 4096) return fail(SD_ERR_UNSUPPORTED, "more than 4096 grouping sets");
+    for (int j = g.a; j < g.a + g.b; j++) {
+      const uint32_t m = (uint32_t)p.exprs[j].a;
+      if (p.exprs[j].a < 0 || (n < 32 && (m >> n) != 0)) return fail(SD_ERR_INVALID, "a grouping-set mask has bits at or above the number of GROUP BY expressions");
+      for (uint32_t q : p.sets) if (q == m) return fail(SD_ERR_UNSUPPORTED, "duplicate grouping sets (Expand would feed each row twice into one group)");
+      p.sets.push_back(m);
+    }
+    p.gid_node = p.keys[nk - 1];
+    p.keys.pop_back();
+    return 0;
+  }
+
   int validate() {
     const int ne = (int)p.exprs.size();
     if ((int)p.cols.size() > 64) return fail(SD_ERR_UNSUPPORTED, "more than 64 scan columns in one fused plan");
@@ -208,6 +266,7 @@ struct Gen {
       return fail(SD_ERR_INVALID, "DECIMAL scan column needs 1 <= precision <= 38 and 0 <= scale <= precision");
     for (int i = 0; i < ne; i++) {
       const sd_expr& e = p.exprs[i];
+      if (is_grouping_node(e.op)) continue;   // checked by grouping_sets()
       if (e.op == SD_OP_COL) { if (e.a < 0 || e.a >= (int)p.cols.size()) return fail(SD_ERR_INVALID, "column reference out of range"); }
       else if (e.op == SD_OP_LIT) { if (e.a < 0 || e.a >= (int)p.literal_types.size()) return fail(SD_ERR_INVALID, "literal slot out of range"); }
       else {
@@ -253,6 +312,7 @@ struct Gen {
     auto is_pair = [&](int n) { return p.exprs[n].op == SD_OP_PAIR; };
     for (int i = 0; i < ne; i++) {
       const sd_expr& e = p.exprs[i];
+      if (is_grouping_node(e.op)) continue;
       if (e.op == SD_OP_PAIR && (e.type != SD_DOUBLE || p.exprs[e.a].type != SD_DOUBLE || p.exprs[e.b].type != SD_DOUBLE))
         return fail(SD_ERR_INVALID, "a PAIR node and both its inputs must be DOUBLE (cast them)");
       if (e.op != SD_OP_COL && e.op != SD_OP_LIT && (is_pair(e.a) || (!is_unary(e.op) && is_pair(e.b))))
@@ -277,7 +337,7 @@ struct Gen {
         case SD_OP_COL: n = p.cols[e.a].nullable; break;
         case SD_OP_LIT: n = 1; break;   // a ParamLiteral's value (incl. NULL) is only known at run time
         case SD_OP_DIV: n = 1; break;
-        case SD_OP_ISNULL: case SD_OP_ISNOTNULL: n = 0; break;
+        case SD_OP_ISNULL: case SD_OP_ISNOTNULL: case SD_OP_GROUPING_SET: case SD_OP_GROUPING_ID: n = 0; break;
         case SD_OP_CAST: n = p.expr_nullable[e.a] || e.type == SD_DECIMAL; break;   // Cast.forceNullable: -> DECIMAL may overflow to NULL
         case SD_OP_NEG: case SD_OP_NOT: n = p.expr_nullable[e.a]; break;
         case SD_OP_IN: n = 1; break;
@@ -888,6 +948,7 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
   out.cols.assign(d->cols, d->cols + d->ncols);
   out.exprs.assign(d->exprs, d->exprs + d->nexprs);
   out.keys.assign(d->keys, d->keys + d->nkeys);
+  out.desc_keys = out.keys;
   out.aggs.assign(d->aggs, d->aggs + d->naggs);
   out.proj.assign(d->proj, d->proj + d->nproj);
   out.literal_types.assign(d->literal_types, d->literal_types + d->nliterals);
@@ -895,7 +956,9 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
   const bool mutate = (d->flags & SD_PLAN_MUTATE) != 0;
   out.flags = mutate ? SD_PLAN_MUTATE : 0;
   Gen g(out, err);
-  int rc = g.validate();
+  int rc = g.grouping_sets();
+  if (rc) return rc;
+  rc = g.validate();
   if (rc) return rc;
   for (auto& c : out.cols) out.kinds.push_back(kind_of_column(c));
   out.lit_wide.assign(out.literal_types.size(), 0);   // slots read by a wide LIT node or listed by an IN over a wide operand
@@ -959,6 +1022,10 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
     if (out.stages == 0) out.reg_groups = 0;   // the register tables are reduced through the ring's memory
   }
   if (!projection) { rc = g.build_slots(); if (rc) return rc; }
+  if (!out.sets.empty() && out.shifts.size() > (size_t)ROLLUP_MAX_SHIFTS) {
+    err = "grouping sets over more than 16 moment / covariance shifts";
+    return SD_ERR_UNSUPPORTED;
+  }
   if (!out.shifts.empty()) out.reg_groups = 0;   // register tables would need a K lookup per row and group: never built for them
   return g.generate();
 }

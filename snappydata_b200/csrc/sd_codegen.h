@@ -104,6 +104,11 @@ struct PlanSpec {
   std::vector<int32_t> literal_types;
   int filter = -1;
   int flags = 0;                     // sd_plan_desc.flags (SD_PLAN_MUTATE)
+  // grouping sets: the descriptor's last key was this SD_OP_GROUPING_ID node; `keys` are the GROUP BY expressions before it
+  // (the scan kernel is the plain GROUP BY's), `sets` its masks.  -1 / empty otherwise
+  int gid_node = -1;
+  std::vector<uint32_t> sets;
+  int out_keys() const { return (int)keys.size() + (gid_node >= 0 ? 1 : 0); }   // key fields of partial / final rows
   // analysis
   std::vector<int> expr_nullable;
   std::vector<int> kinds;            // K_* per scan column
@@ -124,6 +129,7 @@ struct PlanSpec {
   std::string signature;             // canonical text of everything the generated code depends on
   std::string struct_name;           // Plan_<hash of signature>
   std::string source;                // the generated PLAN struct (CUDA C++)
+  std::vector<int32_t> desc_keys;    // the descriptor's keys (with the GROUPING_ID node)
   sd_plan_desc desc_view() const;    // a descriptor pointing into the vectors above
 };
 

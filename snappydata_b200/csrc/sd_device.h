@@ -61,6 +61,7 @@ constexpr int MAX_LITERALS = 64;
 constexpr int MAX_TABLES = 40;   // per-batch lookup tables (truth tables + key maps) of one plan
 constexpr int MAX_KEYS = 4;        // dense group table (MODE_GROUPS): mixed-radix index over <= 4 dictionary keys
 constexpr int MAX_HASH_KEYS = 32;  // hash table (MODE_HASH): one NULL bit per key in a 32-bit word
+constexpr int ROLLUP_MAX_SHIFTS = 16;   // grouping sets: moment / covariance shifts the roll-up re-centres (sd_rollup.cu)
 
 // One update delta of one column (enc/ColumnDeltaEncoder.scala:300-331): ascending positions +
 // values in the column's normal encoding; null bits index the relative entry.

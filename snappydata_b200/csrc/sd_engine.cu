@@ -402,6 +402,13 @@ struct sd_plan {
   std::vector<uint8_t> finished_rows;   // rows of the last sd_plan_finish (re-served when the caller's buffer was too small)
   int64_t finished_nrows = -1;
   std::vector<Launch> launch_log;
+  // grouping sets: the roll-up table of the fine groups into (keys, gid), and the plan's tables the roll-up kernel reads
+  HashTable rollup = {};
+  uint32_t rollup_capacity = 0;
+  int32_t* d_rollup_meta = nullptr;
+  size_t rollup_meta_cap = 0;
+  double rollup_info[4] = {0, 0, 0, 0};   // sdx_plan_rollup_info
+  cudaEvent_t ev_rollup[2] = {nullptr, nullptr};
   // what every kernel launch since the last reset ran (sdx_plan_launch_log): SDX_LAUNCH_WORDS words per launch
   std::vector<int64_t> launch_records;
   int replay_kind = SDX_REPLAY_NONE;   // why the launches being issued repeat earlier ones
@@ -673,34 +680,58 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
   return 0;
 }
 
+void table_free(HashTable& t) {
+  if (t.state) cudaFree(t.state);
+  if (t.keys) cudaFree(t.keys);
+  if (t.knull) cudaFree(t.knull);
+  if (t.vals) cudaFree(t.vals);
+  if (t.shifts) cudaFree(t.shifts);
+  if (t.overflow) cudaFree(t.overflow);
+  t = HashTable{};
+}
+// device memory of a hash group table of `capacity` entries (state not initialised)
+int table_alloc(HashTable& t, uint32_t capacity, int nk, int ns, int nsh) {
+  table_free(t);
+  SD_CUDA(cudaMalloc(&t.state, (size_t)capacity * 4));
+  SD_CUDA(cudaMalloc(&t.keys, (size_t)capacity * nk * 8));
+  SD_CUDA(cudaMalloc(&t.knull, (size_t)capacity * 4));
+  SD_CUDA(cudaMalloc(&t.vals, (size_t)capacity * ns * 8));
+  if (nsh) SD_CUDA(cudaMalloc(&t.shifts, (size_t)capacity * nsh * 8));
+  SD_CUDA(cudaMalloc(&t.overflow, 1024));   // [0] overflow flag, [8] key count; the rest: diagnostic histograms (SD_EXP_VERIFY builds)
+  SD_CUDA(cudaMemset(t.overflow, 0, 1024));
+  t.count = t.overflow + 8;
+  t.mask = capacity - 1;
+  t.max_probe = std::min<uint32_t>(capacity, 4096);
+  return 0;
+}
 void hash_free(sd_plan* p) {
-  if (p->hash.state) cudaFree(p->hash.state);
-  if (p->hash.keys) cudaFree(p->hash.keys);
-  if (p->hash.knull) cudaFree(p->hash.knull);
-  if (p->hash.vals) cudaFree(p->hash.vals);
-  if (p->hash.shifts) cudaFree(p->hash.shifts);
-  if (p->hash.overflow) cudaFree(p->hash.overflow);
-  p->hash = HashTable{};
+  table_free(p->hash);
   p->hash_capacity = 0;
 }
 
+int hash_ident(sd_plan* p);
 int hash_ensure(sd_plan* p, uint32_t capacity) {
   const int ns = (int)p->spec.slots.size(), nk = std::max<int>(1, (int)p->spec.keys.size());
   if (p->hash_capacity != capacity) {
-    hash_free(p);
-    SD_CUDA(cudaMalloc(&p->hash.state, (size_t)capacity * 4));
-    SD_CUDA(cudaMalloc(&p->hash.keys, (size_t)capacity * nk * 8));
-    SD_CUDA(cudaMalloc(&p->hash.knull, (size_t)capacity * 4));
-    SD_CUDA(cudaMalloc(&p->hash.vals, (size_t)capacity * ns * 8));
-    if (!p->spec.shifts.empty()) SD_CUDA(cudaMalloc(&p->hash.shifts, (size_t)capacity * p->spec.shifts.size() * 8));
-    SD_CUDA(cudaMalloc(&p->hash.overflow, 1024));   // [0] overflow flag, [8] key count; the rest: diagnostic histograms (SD_EXP_VERIFY builds)
-    SD_CUDA(cudaMemset(p->hash.overflow, 0, 1024));
-    p->hash.count = p->hash.overflow + 8;
-    p->hash.mask = capacity - 1;
-    p->hash.max_probe = std::min<uint32_t>(capacity, 4096);
+    p->hash_capacity = 0;
+    int rc = table_alloc(p->hash, capacity, nk, ns, (int)p->spec.shifts.size());
+    if (rc) return rc;
     p->hash_capacity = capacity;
     p->hash_init = false;
   }
+  int rc = hash_ident(p);
+  if (rc) return rc;
+  if (!p->hash_init) {
+    rc = hash_table_init(p->stream, p->hash, capacity, ns, p->d_hash_ident, (int)p->spec.shifts.size());
+    if (rc) return rc;
+    p->hash_init = true;
+  }
+  return 0;
+}
+
+// the slot identities a hash group table starts from (device copy, made once)
+int hash_ident(sd_plan* p) {
+  const int ns = (int)p->spec.slots.size();
   if (!p->d_hash_ident) {
     std::vector<uint64_t> id(ns);
     for (int s = 0; s < ns; s++) {
@@ -710,11 +741,6 @@ int hash_ensure(sd_plan* p, uint32_t capacity) {
     }
     SD_CUDA(cudaMalloc(&p->d_hash_ident, (size_t)std::max(ns, 1) * 8));
     SD_CUDA(cudaMemcpy(p->d_hash_ident, id.data(), (size_t)ns * 8, cudaMemcpyHostToDevice));
-  }
-  if (!p->hash_init) {
-    int rc = hash_table_init(p->stream, p->hash, capacity, ns, p->d_hash_ident, (int)p->spec.shifts.size());
-    if (rc) return rc;
-    p->hash_init = true;
   }
   return 0;
 }
@@ -1299,6 +1325,168 @@ void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, const uint64_t* k
   }
 }
 
+// compacted entries of a hash group table on the device: keys [count][nk], knull, vals [count][ns], K words [count][nsh]
+struct Entries {
+  int64_t* keys = nullptr; uint32_t* knull = nullptr; uint64_t* vals = nullptr; uint64_t* shifts = nullptr; uint32_t* cursor = nullptr;
+  uint32_t count = 0;
+  void release() {
+    if (keys) cudaFree(keys);
+    if (knull) cudaFree(knull);
+    if (vals) cudaFree(vals);
+    if (shifts) cudaFree(shifts);
+    if (cursor) cudaFree(cursor);
+    *this = Entries();
+  }
+};
+int compact_entries(sd_plan* p, const HashTable& t, uint32_t capacity, int nk, int ns, int nsh, uint32_t count, Entries& out) {
+  const size_t n = std::max<uint32_t>(count, 1);
+  out.count = count;
+  SD_CUDA(cudaMalloc(&out.keys, n * std::max(nk, 1) * 8));
+  SD_CUDA(cudaMalloc(&out.knull, n * 4));
+  SD_CUDA(cudaMalloc(&out.vals, n * ns * 8));
+  SD_CUDA(cudaMalloc(&out.cursor, 64));
+  if (nsh) SD_CUDA(cudaMalloc(&out.shifts, n * nsh * 8));
+  return hash_table_compact(p->stream, t, capacity, nk, ns, out.keys, out.knull, out.vals, out.cursor, nsh, out.shifts);
+}
+
+// compacted entries -> partial rows in p->finished_rows.  A key word is the value's code, the address of its record (STRING /
+// wide DECIMAL keys of the hash table), or -- dict_keys, the roll-up of a dense table -- the query-global dictionary id of a
+// STRING key.  Entries of a grouping-sets roll-up carry gid as their last key word.
+int emit_entries(sd_plan* p, const Entries& d, int nk, bool dict_keys) {
+  const PlanSpec& sp = p->spec;
+  const int ns = (int)sp.slots.size(), nsh = (int)sp.shifts.size(), nscan = (int)sp.keys.size();
+  const uint32_t count = d.count;
+  std::vector<int64_t> hk((size_t)count * nk);
+  std::vector<uint32_t> hn(count);
+  std::vector<uint64_t> hv((size_t)count * ns), hs((size_t)count * nsh);
+  if (count) {
+    if (nsh) SD_CUDA(cudaMemcpyAsync(hs.data(), d.shifts, hs.size() * 8, cudaMemcpyDeviceToHost, p->stream));
+    SD_CUDA(cudaMemcpyAsync(hk.data(), d.keys, hk.size() * 8, cudaMemcpyDeviceToHost, p->stream));
+    SD_CUDA(cudaMemcpyAsync(hn.data(), d.knull, hn.size() * 4, cudaMemcpyDeviceToHost, p->stream));
+    SD_CUDA(cudaMemcpyAsync(hv.data(), d.vals, hv.size() * 8, cudaMemcpyDeviceToHost, p->stream));
+  }
+  SD_CUDA(cudaStreamSynchronize(p->stream));
+  // STRING keys are held by reference (address of the [len][bytes] record in a resident buffer): fetch their bytes
+  std::vector<std::vector<std::string>> key_strings((size_t)nk);
+  for (int k = 0; k < nscan && count && !dict_keys; k++) {
+    if (sp.exprs[sp.keys[k]].type != SD_STRING && !node_is_wide(sp, sp.keys[k])) continue;
+    int rc = fetch_string_records(p->stream, d.keys + k, (int64_t)count, nk, key_strings[(size_t)k]);
+    if (rc) return rc;
+  }
+  const std::vector<int> types = partial_field_types(sp);
+  StrMap agg_strs;
+  int rc = fetch_agg_strings(p, hv.data(), count, agg_strs);
+  if (rc) return rc;
+  std::vector<uint8_t>& out = p->finished_rows;
+  out.clear();
+  for (uint32_t g = 0; g < count; g++) {
+    std::vector<HVal> vals;
+    for (int k = 0; k < nk; k++) {
+      HVal v;
+      const int64_t code = hk[(size_t)g * nk + k];
+      if ((hn[g] >> k) & 1u) v.isnull = true;
+      else if (dict_keys && k < nscan) v.s = p->key_vals[(size_t)k][(size_t)code];
+      else if (types[k] == SD_STRING) v.s = key_strings[(size_t)k][g];
+      else if (!key_strings[(size_t)k].empty()) {   // wide DECIMAL key held by reference
+        const std::string& b = key_strings[(size_t)k][g];
+        if (b.empty() || b.size() > 16) return set_error(SD_ERR_CUDA, "corrupt DECIMAL key record (%zu bytes)", b.size());
+        v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(b.data()), b.size()); v.i = (int64_t)v.w;
+      }
+      else if (type_is_fp(types[k])) memcpy(&v.d, &code, 8);
+      else { v.i = code; v.w = code; }
+      vals.push_back(v);
+    }
+    append_agg_fields(sp, &hv[(size_t)g * ns], nsh ? &hs[(size_t)g * nsh] : nullptr, vals, &agg_strs);
+    emit_unsafe_row(out, types, vals);
+  }
+  p->finished_nrows = count;
+  return 0;
+}
+
+// grouping sets: the fine groups in `a` (compacted hash entries, or the dense table when a.keys is null) rolled up into
+// (keys, gid) on the device, then emitted.  The roll-up table starts at 2 x fine x sets entries -- a bound on the coarse
+// groups, so it overflows only when an insert exhausts its probe budget; it then grows and the roll-up runs again (the scan is
+// not replayed).
+int rollup_rows(sd_plan* p, RollupArgs a, uint32_t fine_groups) {
+  const PlanSpec& sp = p->spec;
+  const int ns = (int)sp.slots.size(), nsh = (int)sp.shifts.size(), nk = (int)sp.keys.size();
+  // the plan's tables: masks, slot ops, slot roles, per shift its n slot and S_j slots, per pair its two shifts
+  std::vector<int32_t> meta;
+  auto put = [&](const std::vector<int32_t>& v) { const size_t o = meta.size(); meta.insert(meta.end(), v.begin(), v.end()); return o; };
+  std::vector<int32_t> masks(sp.sets.begin(), sp.sets.end()), ops(ns), roles(ns, -1);
+  std::vector<int32_t> cnt((size_t)std::max(nsh, 1), 0), pows((size_t)std::max(nsh, 1) * 4, 0);
+  std::vector<int32_t> px(std::max<size_t>(sp.pairs.size(), 1), 0), py(px.size(), 0);
+  for (int s = 0; s < ns; s++) ops[s] = sp.slots[s].op;
+  for (int i = 0; i < nsh; i++)
+    for (int j = 1; j <= sp.shifts[i].order; j++) {
+      roles[sp.shifts[i].pow_slot[j - 1]] = (i << 3) | j;
+      pows[(size_t)i * 4 + j - 1] = sp.shifts[i].pow_slot[j - 1];
+    }
+  for (size_t q = 0; q < sp.pairs.size(); q++) { roles[sp.pairs[q].xy_slot] = -2 - (int)q; px[q] = sp.pairs[q].shift_x; py[q] = sp.pairs[q].shift_y; }
+  for (auto& m : sp.agg_map) {   // n of a shift's input: its aggregate's count slot
+    if (m.shift >= 0) cnt[m.shift] = m.count_slot;
+    if (m.shift_y >= 0) cnt[m.shift_y] = m.count_slot;
+  }
+  const size_t o_masks = put(masks), o_ops = put(ops), o_roles = put(roles), o_cnt = put(cnt), o_pows = put(pows), o_px = put(px), o_py = put(py);
+  if (meta.size() > p->rollup_meta_cap) {
+    if (p->d_rollup_meta) cudaFree(p->d_rollup_meta);
+    p->d_rollup_meta = nullptr;
+    p->rollup_meta_cap = 0;
+    SD_CUDA(cudaMalloc(&p->d_rollup_meta, meta.size() * 4));
+    p->rollup_meta_cap = meta.size();
+  }
+  SD_CUDA(cudaMemcpyAsync(p->d_rollup_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, p->stream));
+  a.masks = reinterpret_cast<const uint32_t*>(p->d_rollup_meta + o_masks);
+  a.slot_op = p->d_rollup_meta + o_ops; a.slot_role = p->d_rollup_meta + o_roles;
+  a.shift_count = p->d_rollup_meta + o_cnt; a.shift_pow = p->d_rollup_meta + o_pows;
+  a.pair_x = p->d_rollup_meta + o_px; a.pair_y = p->d_rollup_meta + o_py;
+  a.nk = nk; a.ns = ns; a.nsh = nsh; a.nsets = (int)sp.sets.size(); a.rows_slot = sp.rows_slot;
+  int rc = hash_ident(p);
+  if (rc) return rc;
+  constexpr uint32_t CAP_MAX = 1u << 28;
+  const uint64_t want = std::max<uint64_t>(2ull * a.nfine * (uint64_t)a.nsets, 1024);
+  uint32_t cap = 1024;
+  while (cap < want && cap < CAP_MAX) cap *= 2;
+  if (const char* e = getenv("SD_TUNE_ROLLUP_CAP")) {   // first capacity (tests: the growth path)
+    const long v = atol(e);
+    if (v >= 16 && (v & (v - 1)) == 0 && v <= (long)CAP_MAX) cap = (uint32_t)v;
+  }
+  double ms = 0;
+  int launches = 0;
+  uint32_t flags[16];
+  for (;;) {
+    if (cap != p->rollup_capacity) {
+      p->rollup_capacity = 0;
+      rc = table_alloc(p->rollup, cap, nk + 1, ns, nsh);
+      if (rc) return rc;
+      p->rollup_capacity = cap;
+    }
+    rc = hash_table_init(p->stream, p->rollup, cap, ns, p->d_hash_ident, nsh);
+    if (rc) return rc;
+    a.out = p->rollup;
+    if (!p->ev_rollup[0]) { SD_CUDA(cudaEventCreate(&p->ev_rollup[0])); SD_CUDA(cudaEventCreate(&p->ev_rollup[1])); }
+    SD_CUDA(cudaEventRecord(p->ev_rollup[0], p->stream));
+    rc = rollup_launch(p->stream, a);
+    if (rc) return rc;
+    SD_CUDA(cudaEventRecord(p->ev_rollup[1], p->stream));
+    launches++;
+    SD_CUDA(cudaMemcpyAsync(flags, p->rollup.overflow, 64, cudaMemcpyDeviceToHost, p->stream));
+    SD_CUDA(cudaStreamSynchronize(p->stream));
+    float lms = 0;
+    if (cudaEventElapsedTime(&lms, p->ev_rollup[0], p->ev_rollup[1]) == cudaSuccess) ms += lms;
+    if (!flags[0]) break;
+    if (cap >= CAP_MAX) return set_error(SD_ERR_UNSUPPORTED, "grouping-sets roll-up table would exceed 2^28 entries");
+    cap *= 2;
+  }
+  Entries c;
+  rc = compact_entries(p, p->rollup, p->rollup_capacity, nk + 1, ns, nsh, flags[8], c);
+  if (rc) { c.release(); return rc; }
+  p->rollup_info[0] = ms; p->rollup_info[1] = fine_groups; p->rollup_info[2] = flags[8]; p->rollup_info[3] = launches;
+  rc = emit_entries(p, c, nk + 1, a.keys == nullptr);
+  c.release();
+  return rc;
+}
+
 // MODE_HASH: grow + replay on overflow, compact the occupied entries, emit partial rows
 int finish_hash(sd_plan* p) {
   const PlanSpec& sp = p->spec;
@@ -1322,26 +1510,10 @@ int finish_hash(sd_plan* p) {
     p->replay_kind = SDX_REPLAY_NONE;
   }
   const uint32_t count = flags[8];
-  // compact -> host
-  int64_t* d_keys = nullptr; uint32_t* d_knull = nullptr; uint64_t* d_vals = nullptr; uint32_t* d_cursor = nullptr; uint64_t* d_shifts = nullptr;
-  const size_t n = std::max<uint32_t>(count, 1);
-  SD_CUDA(cudaMalloc(&d_keys, n * std::max(nk, 1) * 8));
-  SD_CUDA(cudaMalloc(&d_knull, n * 4));
-  SD_CUDA(cudaMalloc(&d_vals, n * ns * 8));
-  SD_CUDA(cudaMalloc(&d_cursor, 64));
-  if (nsh) SD_CUDA(cudaMalloc(&d_shifts, n * nsh * 8));
-  int rc = hash_table_compact(p->stream, p->hash, p->hash_capacity, nk, ns, d_keys, d_knull, d_vals, d_cursor, nsh, d_shifts);
+  Entries f;
+  int rc = compact_entries(p, p->hash, p->hash_capacity, nk, ns, nsh, count, f);
   if (rc) return rc;
-  std::vector<int64_t> hk((size_t)count * nk);
-  std::vector<uint32_t> hn(count);
-  std::vector<uint64_t> hv((size_t)count * ns), hs((size_t)count * nsh);
   unsigned long long counters[2] = {0, 0};
-  if (count) {
-    if (nsh) SD_CUDA(cudaMemcpyAsync(hs.data(), d_shifts, hs.size() * 8, cudaMemcpyDeviceToHost, p->stream));
-    SD_CUDA(cudaMemcpyAsync(hk.data(), d_keys, hk.size() * 8, cudaMemcpyDeviceToHost, p->stream));
-    SD_CUDA(cudaMemcpyAsync(hn.data(), d_knull, hn.size() * 4, cudaMemcpyDeviceToHost, p->stream));
-    SD_CUDA(cudaMemcpyAsync(hv.data(), d_vals, hv.size() * 8, cudaMemcpyDeviceToHost, p->stream));
-  }
   SD_CUDA(cudaMemcpyAsync(counters, p->d_counters, 16, cudaMemcpyDeviceToHost, p->stream));
   SD_CUDA(cudaStreamSynchronize(p->stream));
   if (getenv("SD_DEBUG_VERIFY")) {   // diagnostic builds (SD_JIT_DEFINES=-DSD_EXP_VERIFY=1): staged tile vs global memory
@@ -1361,45 +1533,24 @@ int finish_hash(sd_plan* p) {
     fprintf(stderr, "[verify] mismatching values %llu; first: column %llu stage %llu row %llu staged %016llx true %016llx\n", dbg[4],
             (dbg[5] >> 56) - (dbg[5] ? 1 : 0), (dbg[5] >> 48) & 0xff, dbg[5] & 0xffffffffffffull, dbg[6], dbg[7]);
   }
-  // STRING keys are held by reference (address of the [len][bytes] record in a resident buffer): fetch their bytes
-  std::vector<std::vector<std::string>> key_strings((size_t)nk);
-  for (int k = 0; k < nk && count; k++) {
-    if (sp.exprs[sp.keys[k]].type != SD_STRING && !node_is_wide(sp, sp.keys[k])) continue;
-    rc = fetch_string_records(p->stream, d_keys + k, (int64_t)count, nk, key_strings[(size_t)k]);
-    if (rc) { cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor); if (d_shifts) cudaFree(d_shifts); return rc; }
-  }
-  cudaFree(d_keys); cudaFree(d_knull); cudaFree(d_vals); cudaFree(d_cursor); if (d_shifts) cudaFree(d_shifts);
   update_agg_time(p);
   p->metrics[6] = (int64_t)(p->agg_ms * 1e6);
   p->metrics[8] = (int64_t)counters[0];
   p->metrics[11] = (int64_t)counters[0];
-  const std::vector<int> types = partial_field_types(sp);
-  StrMap agg_strs;
-  rc = fetch_agg_strings(p, hv.data(), count, agg_strs);
-  if (rc) return rc;
-  std::vector<uint8_t>& out = p->finished_rows;
-  out.clear();
-  for (uint32_t g = 0; g < count; g++) {
-    std::vector<HVal> vals;
-    for (int k = 0; k < nk; k++) {
-      HVal v;
-      const int64_t code = hk[(size_t)g * nk + k];
-      if ((hn[g] >> k) & 1u) v.isnull = true;
-      else if (types[k] == SD_STRING) v.s = key_strings[(size_t)k][g];
-      else if (!key_strings[(size_t)k].empty()) {   // wide DECIMAL key held by reference
-        const std::string& b = key_strings[(size_t)k][g];
-        if (b.empty() || b.size() > 16) return set_error(SD_ERR_CUDA, "corrupt DECIMAL key record (%zu bytes)", b.size());
-        v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(b.data()), b.size()); v.i = (int64_t)v.w;
-      }
-      else if (type_is_fp(types[k])) memcpy(&v.d, &code, 8);
-      else { v.i = code; v.w = code; }
-      vals.push_back(v);
-    }
-    append_agg_fields(sp, &hv[(size_t)g * ns], nsh ? &hs[(size_t)g * nsh] : nullptr, vals, &agg_strs);
-    emit_unsafe_row(out, types, vals);
+  if (!sp.sets.empty()) {
+    RollupArgs a;
+    memset(&a, 0, sizeof(a));
+    a.keys = f.keys; a.knull = f.knull; a.vals = f.vals; a.shifts = f.shifts;
+    a.nfine = count;
+    for (int k = 0; k < nk; k++)
+      if (sp.exprs[sp.keys[k]].type == SD_STRING || node_is_wide(sp, sp.keys[k])) a.strmask |= 1u << k;
+    rc = rollup_rows(p, a, count);
+    f.release();
+    return rc;
   }
-  p->finished_nrows = count;
-  return 0;
+  rc = emit_entries(p, f, nk, false);
+  f.release();
+  return rc;
 }
 
 // MODE_PROJECT: grow + replay when the record buffer was too small, then records -> UnsafeRows
@@ -2063,6 +2214,17 @@ static int finish_dense(sd_plan* p) {
   p->metrics[6] = (int64_t)(p->agg_ms * 1e6);
   p->metrics[8] = (int64_t)counters[0];
   p->metrics[11] = (int64_t)counters[0];
+  if (!sp.sets.empty()) {   // roll the dense table's groups up into (keys, gid)
+    RollupArgs a;
+    memset(&a, 0, sizeof(a));
+    a.vals = p->d_result;
+    a.shifts = p->d_result + (size_t)p->ngroups * ns;
+    a.nfine = (uint32_t)p->ngroups;
+    for (size_t k = 0; k < sp.keys.size(); k++) { a.radix[k] = p->radix[k]; a.null_id[k] = p->key_null_id[k]; }
+    uint32_t fine = 0;
+    for (int g = 0; g < p->ngroups; g++) fine += h[(size_t)g * ns + sp.rows_slot] != 0;
+    return rollup_rows(p, a, fine);
+  }
   StrMap agg_strs;
   {
     std::vector<uint64_t> copy(h, h + ne);   // (the pinned mirror is reused by the fetch's own read-backs)
@@ -2132,6 +2294,7 @@ int sd_plan_reset(sd_plan* p) {
   p->exec_batches.clear();
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
+  memset(p->rollup_info, 0, sizeof(p->rollup_info));
   if (p->d_out_count) SD_CUDA(cudaMemsetAsync(p->d_out_count, 0, 8, p->stream));
   p->have_timing = false;
   p->ev_used = 0;
@@ -2163,6 +2326,12 @@ int sd_plan_metrics(sd_plan* p, int64_t out[SD_NUM_METRICS]) {
   return 0;
 }
 
+int sdx_plan_rollup_info(sd_plan* p, double out[4]) {
+  if (!p || !out) return set_error(SD_ERR_INVALID, "sdx_plan_rollup_info: null argument");
+  memcpy(out, p->rollup_info, sizeof(p->rollup_info));
+  return 0;
+}
+
 int sdx_plan_launch_log(sd_plan* p, int64_t* out, int32_t cap, int32_t* n) {
   if (!p || !n || cap < 0 || (cap > 0 && !out)) return set_error(SD_ERR_INVALID, "sdx_plan_launch_log: bad arguments");
   const int32_t have = (int32_t)(p->launch_records.size() / SDX_LAUNCH_WORDS);
@@ -2185,6 +2354,9 @@ void sd_plan_destroy(sd_plan* p) {
   if (p->h_pinned) cudaFreeHost(p->h_pinned);
   if (p->d_partials) cudaFree(p->d_partials);
   hash_free(p);
+  table_free(p->rollup);
+  if (p->d_rollup_meta) cudaFree(p->d_rollup_meta);
+  if (p->ev_rollup[0]) { cudaEventDestroy(p->ev_rollup[0]); cudaEventDestroy(p->ev_rollup[1]); }
   if (p->d_out) cudaFree(p->d_out);
   if (p->h_recs) cudaFreeHost(p->h_recs);
   p->roww.release();
@@ -2200,6 +2372,7 @@ void sd_plan_destroy(sd_plan* p) {
 int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32_t* slot_is_f64) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_partials_layout: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
+  if (!p->spec.sets.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: a grouping-sets plan has no dense partials");
   if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: shifted sums (moments, covariance) of different GPUs do not add");
   const int ns = (int)p->spec.slots.size();
   if (ngroups) *ngroups = p->ngroups;
@@ -2211,6 +2384,7 @@ int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_export_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_out) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
+  if (!p->spec.sets.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: a grouping-sets plan has no dense partials");
   if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: shifted sums (moments, covariance) of different GPUs do not add");
   SD_CUDA(cudaSetDevice(p->device));
   int rc = flush_pending(p);
@@ -2225,6 +2399,7 @@ int sd_plan_import_partials(sd_plan* p, const void* dev_in, int64_t bytes) {
   if (p && p->spec.mode == MODE_MUTATE) return set_error(SD_ERR_STATE, "sd_plan_import_partials: an UPDATE / DELETE plan keeps no result rows or partials");
   if (!p || !dev_in) return set_error(SD_ERR_INVALID, "null argument");
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
+  if (!p->spec.sets.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: a grouping-sets plan has no dense partials");
   if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: shifted sums (moments, covariance) of different GPUs do not add");
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
@@ -2428,7 +2603,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
     if (out_nrows) *out_nrows = n;
     return 0;
   }
-  const int nk = (int)sp.keys.size();
+  const int nk = sp.out_keys();
   const std::vector<int> types = partial_field_types(sp);
   const int n = (int)types.size();
   struct Group { std::vector<HVal> keys; std::vector<HVal> bufs; };
@@ -2647,6 +2822,7 @@ static bool dense_exchange_eligible(const sd_plan* p) {
   const PlanSpec& sp = p->spec;
   if (sp.mode != MODE_NOKEY && sp.mode != MODE_GROUPS) return false;
   if (p->finished_nrows >= 0) return false;   // rows already materialised by an earlier call
+  if (!sp.sets.empty()) return false;         // the ranks' rolled-up rows are gathered and merged by (keys, gid)
   for (const auto& sl : sp.slots) if (sl.op == SLOT_MIN_STR || sl.op == SLOT_MAX_STR || sl.op == SLOT_MIN_DEC || sl.op == SLOT_MAX_DEC) return false;
   // limb sums are exact below 2^31 rows of ONE execution: summing them over the ranks could pass 2^64, so wide-DECIMAL sums
   // take the by-value exchange, whose merge adds recombined 128-bit totals with an overflow check

@@ -60,6 +60,32 @@ int jit_compile(const PlanSpec& spec, int device, KernelEntry& out);
 int hash_table_init(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nslot, const uint64_t* d_ident, int nshift);
 int hash_table_compact(cudaStream_t stream, const HashTable& t, uint32_t capacity, int nk, int nslot, int64_t* out_keys,
                        uint32_t* out_knull, uint64_t* out_vals, uint32_t* d_cursor, int nshift, uint64_t* out_shifts);
+// ---- grouping-sets roll-up (sd_rollup.cu): fine groups of the plain GROUP BY scan -> a hash table keyed by (keys, gid) ---------
+struct RollupArgs {
+  // fine groups: compacted hash entries (keys != nullptr: keys [nfine][nk], knull) or the dense [nfine][ns] table (keys == nullptr:
+  // entry e is the mixed-radix index over radix[], dictionary id null_id[k] is key k's NULL)
+  const int64_t* keys;
+  const uint32_t* knull;
+  const uint64_t* vals;          // [nfine][ns]
+  const uint64_t* shifts;        // [nfine][nsh] K words
+  int32_t radix[MAX_KEYS];
+  int32_t null_id[MAX_KEYS];
+  uint32_t nfine;
+  int32_t nk, ns, nsh;
+  int32_t rows_slot;             // an entry whose row count is 0 does not exist
+  uint32_t strmask;              // keys held by reference (compared by their bytes)
+  const uint32_t* masks;         // [nsets]
+  int32_t nsets;
+  const int32_t* slot_op;        // [ns] SLOT_*
+  const int32_t* slot_role;      // [ns] -1 plain; (shift << 3) | j: S_j of a shift; -2 - q: S_xy of pair q
+  const int32_t* shift_count;    // [nsh] the slot holding n of the shift's input
+  const int32_t* shift_pow;      // [nsh][4] S_1..S_4 slots
+  const int32_t* pair_x;         // [npair] shift of x
+  const int32_t* pair_y;         // [npair] shift of y
+  HashTable out;                 // nk + 1 keys (the last is gid), ns slots, nsh K words per entry
+};
+int rollup_launch(cudaStream_t stream, const RollupArgs& a);
+
 // strings held by reference -> host: d_recs[i * stride] = device address of a [len:int32][bytes] record (0: none)
 int fetch_string_records(cudaStream_t stream, const int64_t* d_recs, int64_t n, int64_t stride, std::vector<std::string>& out);
 

@@ -191,12 +191,13 @@ __device__ __forceinline__ uint64_t hash_mix64(uint64_t h, uint64_t v) {
 // hashed and compared by its bytes
 __device__ __forceinline__ uint32_t ld_relaxed_u32(const uint32_t* p) { uint32_t v; asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ int64_t ld_relaxed_s64(const int64_t* p) { int64_t v; asm volatile("ld.relaxed.gpu.global.s64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v; }
-template <int NK, uint32_t STRMASK>
-__device__ __forceinline__ int64_t hash_find_or_insert(const HashTable& t, const int64_t* kc, uint32_t knull) {
+// The probe / compare / publish protocol of every hash group table (the scan's and the grouping-sets roll-up's, sd_rollup.cu):
+// nk keys, strmask as STRMASK above.  The scan passes compile-time constants, so its loops unroll as before.
+__device__ __forceinline__ int64_t hash_probe(const HashTable& t, const int64_t* kc, uint32_t knull, int nk, uint32_t strmask) {
   uint64_t h = 0x2545f4914f6cdd1dull ^ knull;
 #pragma unroll
-  for (int k = 0; k < NK; k++) {
-    if ((STRMASK >> k) & 1u) h = hash_mix64(h, kc[k] ? str_hash_rec(reinterpret_cast<const uint8_t*>(kc[k])) : 0ull);
+  for (int k = 0; k < nk; k++) {
+    if ((strmask >> k) & 1u) h = hash_mix64(h, kc[k] ? str_hash_rec(reinterpret_cast<const uint8_t*>(kc[k])) : 0ull);
     else h = hash_mix64(h, (uint64_t)kc[k]);
   }
   uint32_t pos = (uint32_t)h & t.mask;
@@ -206,7 +207,7 @@ __device__ __forceinline__ int64_t hash_find_or_insert(const HashTable& t, const
       st = atomicCAS(&t.state[pos], 0u, 1u);
       if (st == 0u) {   // we own the entry: publish the key, then mark it full
 #pragma unroll
-        for (int k = 0; k < NK; k++) t.keys[(size_t)pos * NK + k] = kc[k];
+        for (int k = 0; k < nk; k++) t.keys[(size_t)pos * nk + k] = kc[k];
         t.knull[pos] = knull;
         __threadfence();
         *reinterpret_cast<volatile uint32_t*>(&t.state[pos]) = 2u;
@@ -221,15 +222,19 @@ __device__ __forceinline__ int64_t hash_find_or_insert(const HashTable& t, const
     const size_t dep = (size_t)(st - 2u);   // 0; not known to the compiler
     bool same = ld_relaxed_u32(&t.knull[pos + dep]) == knull;
 #pragma unroll
-    for (int k = 0; k < NK; k++) {
-      const int64_t have = ld_relaxed_s64(&t.keys[(size_t)pos * NK + k + dep]);
-      if ((STRMASK >> k) & 1u) same = same && (have == kc[k] || (have && kc[k] && str_eq_recs(reinterpret_cast<const uint8_t*>(have), reinterpret_cast<const uint8_t*>(kc[k]))));
+    for (int k = 0; k < nk; k++) {
+      const int64_t have = ld_relaxed_s64(&t.keys[(size_t)pos * nk + k + dep]);
+      if ((strmask >> k) & 1u) same = same && (have == kc[k] || (have && kc[k] && str_eq_recs(reinterpret_cast<const uint8_t*>(have), reinterpret_cast<const uint8_t*>(kc[k]))));
       else same = same && have == kc[k];
     }
     if (same) return pos;
   }
   atomicExch(t.overflow, 1u);
   return -1;
+}
+template <int NK, uint32_t STRMASK>
+__device__ __forceinline__ int64_t hash_find_or_insert(const HashTable& t, const int64_t* kc, uint32_t knull) {
+  return hash_probe(t, kc, knull, NK, STRMASK);
 }
 
 // ---- moment aggregates: sums S_j = sum (x - K)^j around one shift K per group ---------------------------------------------

@@ -70,6 +70,7 @@ class PlanBuilder:
         self.literal_types: List[SqlType] = []
         self._filter: Optional[E] = None
         self._keys: List[E] = []
+        self._sets: Optional[List[int]] = None   # grouping-set masks (rollup / cube / grouping_sets)
         self._aggs: List[Tuple[int, Optional[E]]] = []
         self._proj: List[E] = []
         self._flags = 0
@@ -94,7 +95,35 @@ class PlanBuilder:
                         "with Plan.set_literals (the reference tokenises constants the same way)")
 
     def filter(self, e: E): self._filter = e; return self
-    def group_by(self, *keys: E): self._keys = list(keys); return self
+    def group_by(self, *keys: E): self._keys = list(keys); self._sets = None; return self
+
+    # GROUP BY ... WITH ROLLUP / WITH CUBE / GROUPING SETS: the keys, then spark_grouping_id (an INT key whose value is the set's
+    # mask; bit (n-1-k) set <=> key k is absent, SnappyParser.extractGroupingSet)
+    def grouping_sets(self, keys: Sequence[E], sets: Sequence[Sequence[E]]):
+        """GROUPING SETS: each set is a list of some of `keys` (the others are NULL in its rows)."""
+        keys = list(keys)
+        n = len(keys)
+        masks = []
+        for st in sets:
+            present = {id(e) for e in st}
+            unknown = [e for e in st if all(e is not k for k in keys)]
+            if unknown:
+                raise ValueError("a grouping set may only name GROUP BY expressions")
+            masks.append(sum(1 << (n - 1 - k) for k, e in enumerate(keys) if id(e) not in present))
+        return self.grouping_masks(keys, masks)
+
+    def grouping_masks(self, keys: Sequence[E], masks: Sequence[int]):
+        self._keys = list(keys)
+        self._sets = [int(m) for m in masks]
+        return self
+
+    def rollup(self, *keys: E):
+        n = len(keys)
+        return self.grouping_masks(keys, [(1 << i) - 1 for i in range(n + 1)])
+
+    def cube(self, *keys: E):
+        return self.grouping_masks(keys, list(range(1 << len(keys))))
+
     def agg(self, fn: int, e: Optional[E] = None): self._aggs.append((fn, e)); return self
     def sum(self, e: E): return self.agg(AggFn.SUM, e)
     def avg(self, e: E): return self.agg(AggFn.AVG, e)
@@ -153,6 +182,11 @@ class PlanBuilder:
         keys = [emit(k) for k in self._keys]
         aggs = [(fn, emit(e) if e is not None else -1) for fn, e in self._aggs]
         proj = [emit(p) for p in self._proj]
+        if self._sets is not None:   # appended last: the scan's generated source is the plain GROUP BY's
+            first = len(nodes)
+            nodes.extend((Op.GROUPING_SET, int(SqlType.INT), m, 0, 0) for m in self._sets)
+            nodes.append((Op.GROUPING_ID, int(SqlType.INT), first, len(self._sets), 0))
+            keys.append(len(nodes) - 1)
         return PlanDesc(self.cols, nodes, f, keys, aggs, proj, self.literal_types, self._flags, self._targets)
 
 
