@@ -158,11 +158,25 @@ typedef struct sd_expr {
  * GROUPING_ID list; a GROUPING_ID node that is not the last key, or that is an operand, a filter, an aggregate input, a projection
  * or a SET value; a mask with bits at or above n; b < 1.  SD_ERR_UNSUPPORTED: duplicate masks; n == 0 (no GROUP BY expression
  * before the GROUPING_ID); n > 31; more than 4096 sets; more than 16 moment / covariance shifts (one per distinct moment input,
- * two per distinct PAIR); a GROUPING_ID in an SD_PLAN_MUTATE or projection plan.  These plans have no dense partials export. */
+ * two per distinct PAIR); a GROUPING_ID in an SD_PLAN_MUTATE or projection plan.  These plans have no dense partials export.
+ * FIRST / LAST (Spark 2.1.1 First / Last, restated from upstream Spark; SQL first / first_value / last / last_value, the _IGNORE_NULLS
+ * codes for ignoreNulls = true).  Any input type; a STRING input and a DECIMAL input wider than 18 digits must be a column
+ * (else SD_ERR_UNSUPPORTED).  Buffers, in aggBufferAttributes order: [value of the input type (nullable), valueSet BOOLEAN],
+ * [NULL, false] before any input.  Update, in scan order: FIRST value = valueSet ? value : x, LAST value = x, then valueSet = true;
+ * with ignoreNulls only rows whose x is not NULL count.  Rows the filter rejects and deleted rows do not count; an updated row
+ * counts with its current value.  Scan order of one execution: batches in the order the engine receives them (sd_batch_submit
+ * calls and the row-buffer batch of sd_rows_submit in call order, a store scan in its snapshot's batch order), rows of a batch
+ * in ordinal order.  Merge of partial rows, in the order they are given (sd_partial_merge / sd_final_merge; sd_plan_exchange
+ * merges the ranks in rank order): FIRST value = valueSet1 ? value1 : value2, LAST value = valueSet2 ? value2 : value1,
+ * valueSet = valueSet1 || valueSet2.  The result is value.  The device keeps per group the row with the smallest (FIRST) or
+ * largest (LAST) scan position, whatever order its CTAs run in.  These plans have no dense partials export.  A scan of a batch
+ * whose update delta holds a STRING that the batch's dictionary lacks, under FIRST / LAST of that column, is SD_ERR_UNSUPPORTED
+ * (such a string has no device record; sd_store_compact folds it into the dictionary). */
 typedef enum sd_agg_fn {
   SD_AGG_COUNT_STAR = 1, SD_AGG_COUNT = 2, SD_AGG_SUM = 3, SD_AGG_AVG = 4, SD_AGG_MIN = 5, SD_AGG_MAX = 6,
   SD_AGG_STDDEV_POP = 7, SD_AGG_STDDEV_SAMP = 8, SD_AGG_VAR_POP = 9, SD_AGG_VAR_SAMP = 10, SD_AGG_SKEWNESS = 11,
-  SD_AGG_KURTOSIS = 12, SD_AGG_COVAR_POP = 13, SD_AGG_COVAR_SAMP = 14, SD_AGG_CORR = 15
+  SD_AGG_KURTOSIS = 12, SD_AGG_COVAR_POP = 13, SD_AGG_COVAR_SAMP = 14, SD_AGG_CORR = 15,
+  SD_AGG_FIRST = 16, SD_AGG_LAST = 17, SD_AGG_FIRST_IGNORE_NULLS = 18, SD_AGG_LAST_IGNORE_NULLS = 19
 } sd_agg_fn;
 
 typedef struct sd_agg {

@@ -58,6 +58,8 @@ private[gpu] object Abi {
   final val KURTOSIS = 12
   // Covariance / Corr: two DOUBLE children (ImplicitCastInputTypes casts them), sent as one PAIR node
   final val COVAR_POP = 13; final val COVAR_SAMP = 14; final val CORR = 15
+  // First / Last: the row with the first / last scan position (the row buffer, then the column batches, rows in ordinal order)
+  final val FIRST = 16; final val LAST = 17; final val FIRST_IGNORE_NULLS = 18; final val LAST_IGNORE_NULLS = 19
   // struct sizes / offsets (x86-64; jvm/abi_offsets.txt is generated from the ctypes mirror and checked by the tests)
   final val SIZEOF_COLUMN = 20; final val SIZEOF_EXPR = 20; final val SIZEOF_AGG = 8; final val SIZEOF_DESC = 104
   final val SIZEOF_LITERAL = 40
@@ -288,6 +290,11 @@ object GpuPlanSerializer {
                 case _ => Abi.CORR
               }
               (fn, b.pair(x, y))
+            // first / first_value / last / last_value; Dataset.dropDuplicates(cols) is First(c) per other column
+            case First(c, Literal(ignoreNulls: Boolean, BooleanType)) =>
+              (if (ignoreNulls) Abi.FIRST_IGNORE_NULLS else Abi.FIRST, b.add(c))
+            case Last(c, Literal(ignoreNulls: Boolean, BooleanType)) =>
+              (if (ignoreNulls) Abi.LAST_IGNORE_NULLS else Abi.LAST, b.add(c))
             case f => throw new Unsupported(s"aggregate function ${f.prettyName}")
           }
         }.toArray

@@ -55,12 +55,16 @@ class AggFn:
     STDDEV_POP, STDDEV_SAMP, VAR_POP, VAR_SAMP, SKEWNESS, KURTOSIS = 7, 8, 9, 10, 11, 12
     # two-input aggregates (Spark 2.1.1 Covariance / Corr) over an Op.PAIR node of two DOUBLE inputs
     COVAR_POP, COVAR_SAMP, CORR = 13, 14, 15
+    # Spark 2.1.1 First / Last, with ignoreNulls = false / true
+    FIRST, LAST, FIRST_IGNORE_NULLS, LAST_IGNORE_NULLS = 16, 17, 18, 19
 
 
 # partial buffers of a moment aggregate, all non-nullable DOUBLE: [n, avg, m2] + [m3] (SKEWNESS) + [m3, m4] (KURTOSIS)
 MOMENT_BUFFERS = {AggFn.STDDEV_POP: 3, AggFn.STDDEV_SAMP: 3, AggFn.VAR_POP: 3, AggFn.VAR_SAMP: 3, AggFn.SKEWNESS: 4, AggFn.KURTOSIS: 5}
 # ... and of a two-input aggregate: [n, xAvg, yAvg, ck] + [xMk, yMk] (CORR)
 PAIR_BUFFERS = {AggFn.COVAR_POP: 4, AggFn.COVAR_SAMP: 4, AggFn.CORR: 6}
+# FIRST / LAST: [value of the input type (nullable), valueSet BOOLEAN]
+ORDER_AGGS = (AggFn.FIRST, AggFn.LAST, AggFn.FIRST_IGNORE_NULLS, AggFn.LAST_IGNORE_NULLS)
 
 
 class sd_column(C.Structure):
@@ -402,6 +406,8 @@ class PlanDesc:
                 out += [SqlType.DOUBLE] * MOMENT_BUFFERS[fn]
             elif fn in PAIR_BUFFERS:
                 out += [SqlType.DOUBLE] * PAIR_BUFFERS[fn]
+            elif fn in ORDER_AGGS:
+                out += [self._ftype(e), SqlType.BOOLEAN]
             else:
                 out.append(self._ftype(e))
         return out

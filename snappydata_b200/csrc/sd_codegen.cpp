@@ -43,6 +43,7 @@ std::vector<int> partial_field_types(const PlanSpec& p) {
   for (auto& m : p.agg_map) {
     if (is_moment(m.fn) || is_pair_agg(m.fn)) { t.insert(t.end(), (size_t)agg_buffer_fields(m.fn), SD_DOUBLE); continue; }
     t.push_back(field_type(m.buf_type, m.buf_ps)); if (m.fn == SD_AGG_AVG) t.push_back(SD_LONG);
+    if (is_order_agg(m.fn)) t.push_back(SD_BOOLEAN);   // valueSet
   }
   return t;
 }
@@ -382,7 +383,7 @@ struct Gen {
     for (auto& a : p.aggs) {
       AggMap m;
       memset(&m, 0, sizeof(m));
-      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1; m.shift = -1; m.shift_y = -1;
+      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1; m.shift = -1; m.shift_y = -1; m.order_slot = -1;
       for (int& l : m.limb_slot) l = -1;
       for (int& s : m.pow_slot) s = -1;
       for (int& s : m.pair_slot) s = -1;
@@ -431,6 +432,39 @@ struct Gen {
           sx.pow_slot[1] = m.pair_slot[3];
           sy.pow_slot[1] = m.pair_slot[4];
         }
+        p.agg_map.push_back(m);
+        continue;
+      }
+      if (is_order_agg(a.fn)) {
+        // one (order key, value) pair at an even slot index; FIRST and LAST of one input, or one function with and without
+        // ignoreNulls, keep pairs of their own
+        const bool str = it == SD_STRING, wide = node_is_wide(p, a.expr);
+        if ((str || wide) && p.exprs[a.expr].op != SD_OP_COL)
+          return fail(SD_ERR_UNSUPPORTED, "FIRST / LAST of a STRING or wide DECIMAL expression that is not a column");
+        m.buf_type = it;
+        m.buf_nullable = 1;
+        m.value_slot2 = -1;
+        if (it == SD_DECIMAL) { m.in_ps = decimal_ps(p, a.expr); m.buf_ps = m.in_ps; }
+        const int op = is_last_agg(a.fn) ? SLOT_LAST : SLOT_FIRST;
+        const int gate = a.fn == SD_AGG_FIRST_IGNORE_NULLS || a.fn == SD_AGG_LAST_IGNORE_NULLS ? GATE_ORDER_KEY_IGN : GATE_ORDER_KEY;
+        const std::string in = expr_text(p, a.expr);
+        for (size_t q = 0; q < p.slots.size(); q++)
+          if (p.slots[q].op == op && p.slots[q].gate == gate && expr_text(p, p.slots[q].node) == in) m.order_slot = (int)q;
+        if (m.order_slot < 0) {
+          if (p.slots.size() % 2) p.slots.push_back(SlotSpec{SLOT_ADD_I64, -1, GATE_PAD});
+          m.order_slot = (int)p.slots.size();
+          p.slots.push_back(SlotSpec{op, a.expr, gate});
+          p.slots.push_back(SlotSpec{SLOT_PAIR_VAL, a.expr, GATE_ORDER_VAL});
+          if (str) {   // the value is the address of the row's record, as for MIN / MAX over STRING
+            const int col = p.exprs[a.expr].a;
+            int t = -1;
+            for (size_t ti = 0; ti < p.tables.size(); ti++) if (p.tables[ti].kind == TABLE_KEYPTR && p.tables[ti].col == col && p.tables[ti].key < 0) t = (int)ti;
+            if (t < 0) { p.tables.push_back(TableSpec{TABLE_KEYPTR, col, -1, -1}); t = (int)p.tables.size() - 1; }
+            p.slots.back().table = t;
+          }
+          p.norder++;
+        }
+        m.value_slot = m.order_slot + 1;
         p.agg_map.push_back(m);
         continue;
       }
@@ -521,6 +555,7 @@ struct Gen {
       p.agg_map.push_back(m);
     }
     p.rows_slot = add_slot(SLOT_ADD_I64, -1, GATE_ONE);
+    if (p.norder > 0 && p.slots.size() % 2) p.slots.push_back(SlotSpec{SLOT_ADD_I64, -1, GATE_PAD});   // even group stride
     return 0;
   }
 
@@ -820,7 +855,9 @@ struct Gen {
     for (size_t s = 0; s < p.slots.size(); s++) {
       const SlotSpec& x = p.slots[s];
       sig << (s ? "," : "") << x.op << "/" << x.gate << "/" << (x.node >= 0 ? expr_text(p, x.node) : std::string("-"));
-      if (x.node >= 0 && x.gate != GATE_DECREF) { int rc = emit_node(x.node, done, slt); if (rc) return rc; }
+      const bool order_gate = x.gate == GATE_ORDER_KEY || x.gate == GATE_ORDER_KEY_IGN || x.gate == GATE_ORDER_VAL;
+      const bool by_ref = x.node >= 0 && (x.gate == GATE_DECREF || (order_gate && node_is_wide(p, x.node)));   // record address, not value
+      if (x.node >= 0 && !by_ref) { int rc = emit_node(x.node, done, slt); if (rc) return rc; }
       const std::string V = "v" + std::to_string(x.node), NL = "n" + std::to_string(x.node);
       slt << "    sv[" << s << "] = ";
       if (x.gate == GATE_ONE) slt << "1ull;\n";
@@ -843,6 +880,17 @@ struct Gen {
       else if (x.gate == GATE_PAIR_X) slt << NL << " ? sd::SHIFT_EMPTY : sd::shift_cand(" << V << ");\n";
       else if (x.gate == GATE_PAIR_Y) slt << NL << " ? sd::SHIFT_EMPTY : sd::shift_cand(v" << p.exprs[x.node].b << ");\n";
       else if (x.gate >= GATE_PAIR_XY && x.gate <= GATE_PAIR_YY) slt << "0ull;\n";
+      else if (x.gate == GATE_PAD) slt << "0ull;\n";
+      else if (order_gate) {
+        const int col = p.exprs[x.node].a;
+        const std::string C = std::to_string(col);
+        const std::string isnull = by_ref ? (p.cols[col].nullable ? "r.n" + C : std::string("false")) : NL;
+        if (x.gate == GATE_ORDER_KEY) slt << "ctx.ord | (" << isnull << " ? 1ull : 0ull);\n";
+        else if (x.gate == GATE_ORDER_KEY_IGN) slt << isnull << " ? " << (x.op == SLOT_FIRST ? "0xffffffffffffffffull" : "0ull") << " : ctx.ord;\n";
+        else if (by_ref) slt << isnull << " ? 0ull : (uint64_t)(uintptr_t)(ctx.strbase[" << C << "] + (uint32_t)r.c" << C << ");\n";
+        else if (p.exprs[x.node].type == SD_STRING) slt << isnull << " ? 0ull : (uint64_t)ctx.str_ref(" << C << ", " << x.table << ", r.c" << C << ");\n";
+        else slt << isnull << " ? 0ull : " << (type_is_fp(p.exprs[x.node].type) ? "sd::f2u((double)" + V + ")" : "(uint64_t)(int64_t)" + V) << ";\n";
+      }
       else {
         const bool f = x.op == SLOT_ADD_F64 || x.op == SLOT_MIN_F64 || x.op == SLOT_MAX_F64;
         char ident[32];
@@ -910,6 +958,7 @@ struct Gen {
         for (int j = 1; j <= p.shifts[i].order; j++) o << "(i == " << i << " && j == " << j << ") ? " << p.shifts[i].pow_slot[j - 1] << " : ";
       o << "0; }\n";
     }
+    if (p.norder > 0) o << "  static constexpr int NORDER = " << p.norder << ";\n";   // FIRST / LAST pairs (sd_kernels.cuh PlanOrders)
     if (!p.pairs.empty()) {   // two-input aggregates: S_xy of shifts (x, y) (sd_kernels.cuh apply_shifts)
       const int np = (int)p.pairs.size();
       o << "  static constexpr int NPAIR = " << np << ";\n";
@@ -1027,6 +1076,7 @@ int analyze_plan(const sd_plan_desc* d, PlanSpec& out, std::string& err, const C
     return SD_ERR_UNSUPPORTED;
   }
   if (!out.shifts.empty()) out.reg_groups = 0;   // register tables would need a K lookup per row and group: never built for them
+  if (out.norder > 0) out.reg_groups = 0;        // nor for FIRST / LAST pairs
   return g.generate();
 }
 

@@ -33,10 +33,14 @@ struct TableSpec {
 // GATE_PAIR_X / GATE_PAIR_Y: S_x = sum (x - Kx), S_y = sum (y - Ky) of a two-input aggregate's SD_OP_PAIR node (the row leaves
 // its candidate Kx / Ky there, SHIFT_EMPTY when x or y is NULL); GATE_PAIR_XY: S_xy = sum (x - Kx)(y - Ky); GATE_PAIR_XX /
 // GATE_PAIR_YY: CORR's sum (x - Kx)^2 / sum (y - Ky)^2.  apply_shifts fills them like the moment sums
+// GATE_ORDER_KEY / GATE_ORDER_KEY_IGN: word 0 of a FIRST / LAST pair, the row's order key (sd_device.h ORDER_EMPTY_FIRST) with
+// its NULL flag; _IGN (ignoreNulls): the empty key for a NULL value, so the row does not count.  GATE_ORDER_VAL: word 1, the
+// value (as MIN / MAX store it).  GATE_PAD: an always-zero slot that keeps the pairs at even slot indexes
 enum SlotGate { GATE_VALUE = 0, GATE_NONNULL_COUNT = 1, GATE_ONE = 2, GATE_VALUE_HI32 = 3, GATE_VALUE_LO32 = 4, GATE_STRREF = 5,
                 GATE_LIMB0 = 6, GATE_LIMB1 = 7, GATE_LIMB2 = 8, GATE_LIMB3 = 9, GATE_DECREF = 10,
                 GATE_POW1 = 11, GATE_POW2 = 12, GATE_POW3 = 13, GATE_POW4 = 14,
-                GATE_PAIR_X = 15, GATE_PAIR_Y = 16, GATE_PAIR_XY = 17, GATE_PAIR_XX = 18, GATE_PAIR_YY = 19 };
+                GATE_PAIR_X = 15, GATE_PAIR_Y = 16, GATE_PAIR_XY = 17, GATE_PAIR_XX = 18, GATE_PAIR_YY = 19,
+                GATE_ORDER_KEY = 20, GATE_ORDER_KEY_IGN = 21, GATE_ORDER_VAL = 22, GATE_PAD = 23 };
 
 struct SlotSpec {
   int op;     // SLOT_*
@@ -61,6 +65,7 @@ struct AggMap {
   int pow_slot[4];  // moment aggregate: S_1..S_order; else -1
   int shift_y;      // two-input aggregate: index of its y shift (`shift` is the x shift; count_slot = n, value_slot = S_xy); else -1
   int pair_slot[5]; // two-input aggregate: S_x, S_y, S_xy, S_xx, S_yy (the last two CORR only); else -1
+  int order_slot;   // FIRST / LAST: the pair's key slot (value_slot = order_slot + 1 holds the value); else -1
 };
 
 // a moment aggregate (Spark 2.1.1 CentralMomentAgg): STDDEV_* / VAR_* (order 2), SKEWNESS (3), KURTOSIS (4)
@@ -68,10 +73,13 @@ inline bool is_moment(int fn) { return fn >= SD_AGG_STDDEV_POP && fn <= SD_AGG_K
 inline int moment_order(int fn) { return fn == SD_AGG_KURTOSIS ? 4 : fn == SD_AGG_SKEWNESS ? 3 : 2; }
 // a two-input aggregate (Spark 2.1.1 Covariance / Corr) over an SD_OP_PAIR node
 inline bool is_pair_agg(int fn) { return fn >= SD_AGG_COVAR_POP && fn <= SD_AGG_CORR; }
+// FIRST / LAST with or without ignoreNulls (Spark 2.1.1 First / Last)
+inline bool is_order_agg(int fn) { return fn >= SD_AGG_FIRST && fn <= SD_AGG_LAST_IGNORE_NULLS; }
+inline bool is_last_agg(int fn) { return fn == SD_AGG_LAST || fn == SD_AGG_LAST_IGNORE_NULLS; }
 // partial-row buffer fields of an aggregate: AVG [sum, count]; moments [n, avg, m2, (m3, (m4))]; COVAR_* [n, xAvg, yAvg, ck];
-// CORR [n, xAvg, yAvg, ck, xMk, yMk]; others one
+// CORR [n, xAvg, yAvg, ck, xMk, yMk]; FIRST / LAST [value, valueSet]; others one
 inline int agg_buffer_fields(int fn) {
-  return fn == SD_AGG_AVG ? 2 : is_moment(fn) ? 1 + moment_order(fn) : fn == SD_AGG_CORR ? 6 : is_pair_agg(fn) ? 4 : 1;
+  return fn == SD_AGG_AVG || is_order_agg(fn) ? 2 : is_moment(fn) ? 1 + moment_order(fn) : fn == SD_AGG_CORR ? 6 : is_pair_agg(fn) ? 4 : 1;
 }
 
 // one shift K of a plan's moment sums (its K words are not slots, sd_device.h SHIFT_EMPTY): every moment aggregate over the
@@ -118,6 +126,7 @@ struct PlanSpec {
   std::vector<AggMap> agg_map;
   std::vector<ShiftSpec> shifts;     // moment aggregates' shifts: K words [group][shift] beside the slots
   std::vector<PairSpec> pairs;       // two-input aggregates' cross terms over two of those shifts
+  int norder = 0;                    // FIRST / LAST pairs (sd_device.h SLOT_FIRST)
   int rows_slot = -1;                // COUNT(*)-like slot that tells which groups exist
   int mode = 0;                      // MODE_NOKEY | MODE_GROUPS | MODE_HASH | MODE_PROJECT | MODE_MUTATE
   int rpt = 4;                       // rows per thread per tile (2, 4, 8)

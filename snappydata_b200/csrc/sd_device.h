@@ -167,8 +167,24 @@ enum : int32_t { TABLE_PRIVATE = 0, TABLE_SHARED_ATOMIC = 1, TABLE_GLOBAL_ATOMIC
 // reference down its ObjectHashSet path, SnappyHashAggregateExec.scala:82-94)
 // SLOT_MIN_DEC / SLOT_MAX_DEC: the same for a DECIMAL wider than 18 digits, whose record is [len][big-endian two's-complement
 // unscaled value]; records compare by their numeric value
+// SLOT_FIRST / SLOT_LAST + SLOT_PAIR_VAL: one FIRST / LAST buffer, a pair of adjacent slots at an even slot index (16-byte
+// aligned in every table: the plan's slot count is even too).  Word 0 is the order key of the row the pair holds, word 1 that
+// row's value, stored as MIN / MAX store one (int64, double bits, or the address of a STRING / wide-DECIMAL record).  The pair
+// combines as one unit: the smaller key (FIRST) or the larger key (LAST) wins and the value travels with it.
 enum : int32_t { SLOT_ADD_F64 = 0, SLOT_ADD_I64 = 1, SLOT_MIN_I64 = 2, SLOT_MAX_I64 = 3, SLOT_MIN_F64 = 4, SLOT_MAX_F64 = 5,
-                 SLOT_MIN_STR = 6, SLOT_MAX_STR = 7, SLOT_MIN_DEC = 8, SLOT_MAX_DEC = 9 };
+                 SLOT_MIN_STR = 6, SLOT_MAX_STR = 7, SLOT_MIN_DEC = 8, SLOT_MAX_DEC = 9,
+                 SLOT_FIRST = 10, SLOT_LAST = 11, SLOT_PAIR_VAL = 12 };
+// Order key of a row: ((execution-wide batch sequence + 1) << 32) | (row ordinal << 1) | (1 when the value is NULL).  Unique per
+// row of one execution and increasing in scan order across all its launches (and the same in a launch's replays).  An empty
+// pair holds ORDER_EMPTY_FIRST (FIRST) or 0 (LAST): no row's key takes either, and every row's key beats them.
+constexpr uint64_t ORDER_EMPTY_FIRST = 0xffffffffffffffffull;
+constexpr bool is_order_op(int op) { return op == SLOT_FIRST || op == SLOT_LAST; }
+// initial word of a slot (slot_identity of sd_kernels.cuh, plus the FIRST / LAST order keys), for host and device
+constexpr uint64_t slot_initial(int op) {
+  return op == SLOT_MIN_I64 ? 0x7fffffffffffffffull : op == SLOT_MAX_I64 ? 0x8000000000000000ull
+       : op == SLOT_MIN_F64 ? 0x7ff8000000000000ull : op == SLOT_MAX_F64 ? 0xfff0000000000000ull
+       : op == SLOT_FIRST ? ORDER_EMPTY_FIRST : 0ull;
+}
 
 // Moment aggregates (STDDEV / VARIANCE / SKEWNESS / KURTOSIS) sum S_j = sum (x - K)^j around one shift K per group and input.
 // The K words are not slots: they live beside the running result ([ngroups][NSHIFT] after its [ngroups][NSLOT] entries) and
@@ -198,7 +214,8 @@ struct ScanArgs {
   uint8_t* out_rows;              // MODE_PROJECT: output records
   unsigned long long* out_count;  // MODE_PROJECT: records produced (may exceed out_cap: the host grows and replays)
   int64_t out_cap;                // MODE_PROJECT: capacity in records
-  int32_t batch_base;             // MODE_PROJECT: ordinal of this launch's first batch within the execution
+  int32_t batch_base;             // ordinal of this launch's first batch within the execution (MODE_PROJECT / MODE_MUTATE records;
+                                  // the order keys of FIRST / LAST)
   int32_t chunk_rows;             // rows per work item (multiple of every tile size; default CHUNK_ROWS)
   const uint8_t* lit_pool;        // bytes of the STRING literals of this execution (literal slot k: lits.i[k] = offset << 32 | length);
                                   // a wide DECIMAL literal is its 16-byte little-endian unscaled value there, 16-byte aligned

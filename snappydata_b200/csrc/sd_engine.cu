@@ -473,9 +473,7 @@ int init_result(sd_plan* p, int ngroups) {
   SD_CUDA(cudaStreamSynchronize(p->stream));   // the staging buffer may still be in use by a previous read-back
   uint64_t* hid = p->h_pinned + STATE_HDR;
   for (size_t e = 0; e < ne; e++) {
-    const int op = p->spec.slots[e % ns].op;
-    hid[e] = op == SLOT_MIN_I64 ? 0x7fffffffffffffffull : op == SLOT_MAX_I64 ? 0x8000000000000000ull
-                   : op == SLOT_MIN_F64 ? 0x7ff8000000000000ull : op == SLOT_MAX_F64 ? 0xfff0000000000000ull : 0ull;
+    hid[e] = slot_initial(p->spec.slots[e % ns].op);
   }
   for (size_t e = ne; e < nw; e++) hid[e] = SHIFT_EMPTY;
   SD_CUDA(cudaMemcpyAsync(p->d_result, hid, nw * 8, cudaMemcpyHostToDevice, p->stream));
@@ -635,6 +633,18 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
             aux.push_back((uint8_t)eval_string_predicate(sp, ts.node, s ? s->data() : nullptr, s ? (int)s->size() : 0, p->lits.data()));
           }
         } else if (ts.kind == TABLE_KEYPTR) {   // device address of every code's [len][bytes] record
+          // FIRST / LAST of a STRING column return the winning row's own value: one that exists only in an update delta has no
+          // device record to point at, so the plan is refused rather than answering NULL for it
+          bool order_input = false;
+          for (const auto& m : sp.agg_map)
+            if (m.order_slot >= 0 && sp.slots[(size_t)m.order_slot].node >= 0 && sp.exprs[sp.slots[(size_t)m.order_slot].node].a == ts.col &&
+                m.buf_type == SD_STRING)
+              order_input = true;
+          if (order_input && ts.key < 0)
+            for (int code = n + 1; code < (int)sc.dict_strings.size(); code++)
+              if (code >= (int)sc.dict_rec_ptr.size() || sc.dict_rec_ptr[code] == 0)
+                return set_error(SD_ERR_UNSUPPORTED, "batch %lld: FIRST / LAST of a STRING column whose update deltas hold strings the "
+                                 "batch's dictionary does not (compact the batch first)", (long long)sb.batch_id);
           for (int code = 0; code < ncodes; code++) {
             const int64_t ptr = code < (int)sc.dict_rec_ptr.size() ? sc.dict_rec_ptr[code] : 0;
             aux.insert(aux.end(), reinterpret_cast<const uint8_t*>(&ptr), reinterpret_cast<const uint8_t*>(&ptr) + 8);
@@ -734,11 +744,7 @@ int hash_ident(sd_plan* p) {
   const int ns = (int)p->spec.slots.size();
   if (!p->d_hash_ident) {
     std::vector<uint64_t> id(ns);
-    for (int s = 0; s < ns; s++) {
-      const int op = p->spec.slots[s].op;
-      id[s] = op == SLOT_MIN_I64 ? 0x7fffffffffffffffull : op == SLOT_MAX_I64 ? 0x8000000000000000ull
-            : op == SLOT_MIN_F64 ? 0x7ff8000000000000ull : op == SLOT_MAX_F64 ? 0xfff0000000000000ull : 0ull;
-    }
+    for (int s = 0; s < ns; s++) id[s] = slot_initial(p->spec.slots[s].op);
     SD_CUDA(cudaMalloc(&p->d_hash_ident, (size_t)std::max(ns, 1) * 8));
     SD_CUDA(cudaMemcpy(p->d_hash_ident, id.data(), (size_t)ns * 8, cudaMemcpyHostToDevice));
   }
@@ -859,6 +865,8 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   if (!replay && p->spec.mode != MODE_NOKEY) {
     p->launch_log.push_back({d_batches, d_prefix, nbatches, total_chunks, batch_base, needs_slow, paths});
     if (blist) p->exec_batches.insert(p->exec_batches.end(), blist->begin(), blist->end());
+  } else if (!replay && p->spec.norder > 0 && blist) {   // no keys: only the batch sequence of FIRST / LAST's order keys
+    p->exec_batches.insert(p->exec_batches.end(), blist->begin(), blist->end());
   }
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
@@ -1166,7 +1174,8 @@ int fetch_agg_strings(sd_plan* p, const uint64_t* slots, size_t ngroups, StrMap&
   std::vector<int64_t> ptrs;
   for (auto& m : sp.agg_map) {
     const int op = sp.slots[(size_t)m.value_slot].op;
-    if (m.buf_type != SD_STRING && op != SLOT_MIN_DEC && op != SLOT_MAX_DEC) continue;
+    const bool wide_order = m.order_slot >= 0 && m.buf_type == SD_DECIMAL && (m.buf_ps >> 8) > 18;   // FIRST / LAST: record address
+    if (m.buf_type != SD_STRING && op != SLOT_MIN_DEC && op != SLOT_MAX_DEC && !wide_order) continue;
     for (size_t g = 0; g < ngroups; g++) { const uint64_t a = slots[g * ns + m.value_slot]; if (a && !out.count(a)) { out.emplace(a, std::string()); ptrs.push_back((int64_t)a); } }
   }
   if (ptrs.empty()) return 0;
@@ -1236,6 +1245,23 @@ void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, const uint64_t* k
     HVal v;
     const uint64_t raw = sv[m.value_slot];
     const int64_t cnt = m.count_slot >= 0 ? (int64_t)sv[m.count_slot] : 1;
+    if (m.order_slot >= 0) {   // FIRST / LAST: [value, valueSet] from the pair (order key, value)
+      const uint64_t key = sv[m.order_slot];
+      HVal set;
+      set.i = key != slot_initial(sp.slots[(size_t)m.order_slot].op);
+      if (!set.i || (key & 1ull)) v.isnull = true;   // no row, or the row's value is NULL
+      else if (m.buf_type == SD_STRING || (m.buf_type == SD_DECIMAL && (m.buf_ps >> 8) > 18)) {
+        const auto it = strs ? strs->find(raw) : StrMap::const_iterator();
+        if (!strs || it == strs->end()) v.isnull = true;
+        else if (m.buf_type == SD_STRING) v.s = it->second;
+        else if (it->second.empty() || it->second.size() > 16) v.isnull = true;
+        else { v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(it->second.data()), it->second.size()); v.i = (int64_t)v.w; }
+      } else if (type_is_fp(m.buf_type)) memcpy(&v.d, &raw, 8);
+      else { v.i = (int64_t)raw; v.w = v.i; }
+      vals.push_back(v);
+      vals.push_back(set);
+      continue;
+    }
     if (m.buf_type == SD_STRING) {
       if ((m.buf_nullable && cnt == 0) || raw == 0 || !strs) v.isnull = true;
       else { auto it = strs->find(raw); if (it == strs->end()) v.isnull = true; else v.s = it->second; }
@@ -2374,6 +2400,7 @@ int sd_plan_partials_layout(sd_plan* p, int32_t* ngroups, int32_t* nslots, int32
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
   if (!p->spec.sets.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: a grouping-sets plan has no dense partials");
   if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: shifted sums (moments, covariance) of different GPUs do not add");
+  if (p->spec.norder > 0) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_partials_layout: FIRST / LAST order keys of different GPUs do not compare");
   const int ns = (int)p->spec.slots.size();
   if (ngroups) *ngroups = p->ngroups;
   if (nslots) *nslots = ns;
@@ -2386,6 +2413,7 @@ int sd_plan_export_partials(sd_plan* p, void* dev_out, int64_t cap_bytes) {
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
   if (!p->spec.sets.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: a grouping-sets plan has no dense partials");
   if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: shifted sums (moments, covariance) of different GPUs do not add");
+  if (p->spec.norder > 0) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_export_partials: FIRST / LAST order keys of different GPUs do not compare");
   SD_CUDA(cudaSetDevice(p->device));
   int rc = flush_pending(p);
   if (rc) return rc;
@@ -2401,6 +2429,7 @@ int sd_plan_import_partials(sd_plan* p, const void* dev_in, int64_t bytes) {
   if (p->spec.mode == MODE_HASH || p->spec.mode == MODE_PROJECT) return set_error(SD_ERR_UNSUPPORTED, "dense partials exist only for no-key / dictionary-keyed plans");
   if (!p->spec.sets.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: a grouping-sets plan has no dense partials");
   if (!p->spec.shifts.empty()) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: shifted sums (moments, covariance) of different GPUs do not add");
+  if (p->spec.norder > 0) return set_error(SD_ERR_UNSUPPORTED, "sd_plan_import_partials: FIRST / LAST order keys of different GPUs do not compare");
   p->finished_nrows = -1;
   p->dev_rows_len = -1;
   SD_CUDA(cudaSetDevice(p->device));
@@ -2643,6 +2672,13 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
         const HVal& in = f[nk + k];
         if (is_moment(m.fn)) { moment_merge(&b, &in, moment_order(m.fn)); k += agg_buffer_fields(m.fn); continue; }
         if (is_pair_agg(m.fn)) { pair_merge(&b, &in, m.fn == SD_AGG_CORR); k += agg_buffer_fields(m.fn); continue; }
+        if (is_order_agg(m.fn)) {   // First: valueSet.left ? left : right; Last: valueSet.right ? right : left; valueSet = left || right
+          HVal& bset = g->bufs[k + 1];
+          const HVal& inset = f[nk + k + 1];
+          if (is_last_agg(m.fn) ? inset.i != 0 : bset.i == 0) { b = in; bset.i = bset.i || inset.i; }
+          k += 2;
+          continue;
+        }
         switch (m.fn) {
           case SD_AGG_COUNT_STAR: case SD_AGG_COUNT: b.i += in.i; k++; break;
           case SD_AGG_SUM:
@@ -2673,7 +2709,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
     Group g;
     for (auto& m : sp.agg_map) {
       HVal v;
-      if (m.fn == SD_AGG_SUM || m.fn == SD_AGG_MIN || m.fn == SD_AGG_MAX) v.isnull = true;
+      if (m.fn == SD_AGG_SUM || m.fn == SD_AGG_MIN || m.fn == SD_AGG_MAX || is_order_agg(m.fn)) v.isnull = true;   // FIRST / LAST: [NULL, false]
       g.bufs.push_back(v);
       for (int j = 1; j < agg_buffer_fields(m.fn); j++) g.bufs.push_back(HVal());   // AVG's count, the moments' 0.0s
     }
@@ -2691,6 +2727,7 @@ static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t
       for (auto& m : sp.agg_map) {
         if (is_moment(m.fn)) { vals.push_back(moment_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
         if (is_pair_agg(m.fn)) { vals.push_back(pair_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
+        if (is_order_agg(m.fn)) { vals.push_back(g.bufs[k]); k += 2; continue; }   // First / Last.evaluateExpression: value
         if (m.fn == SD_AGG_AVG) {   // Average.evaluateExpression: sum / count, NULL when count == 0
           HVal v;
           const int64_t cnt = g.bufs[k + 1].i;
@@ -2824,6 +2861,8 @@ static bool dense_exchange_eligible(const sd_plan* p) {
   if (p->finished_nrows >= 0) return false;   // rows already materialised by an earlier call
   if (!sp.sets.empty()) return false;         // the ranks' rolled-up rows are gathered and merged by (keys, gid)
   for (const auto& sl : sp.slots) if (sl.op == SLOT_MIN_STR || sl.op == SLOT_MAX_STR || sl.op == SLOT_MIN_DEC || sl.op == SLOT_MAX_DEC) return false;
+  for (const auto& m : sp.agg_map)   // FIRST / LAST values held as record addresses
+    if (m.order_slot >= 0 && (m.buf_type == SD_STRING || (m.buf_type == SD_DECIMAL && (m.buf_ps >> 8) > 18))) return false;
   // limb sums are exact below 2^31 rows of ONE execution: summing them over the ranks could pass 2^64, so wide-DECIMAL sums
   // take the by-value exchange, whose merge adds recombined 128-bit totals with an overflow check
   for (const auto& sl : sp.slots) if (sl.gate >= GATE_LIMB0 && sl.gate <= GATE_LIMB3) return false;   // values live in this rank's HBM

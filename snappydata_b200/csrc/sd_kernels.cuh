@@ -181,6 +181,70 @@ __device__ __forceinline__ void slot_atomic(int op, uint64_t* p, uint64_t v) {
   }
 }
 
+// ---- FIRST / LAST: (order key, value) pairs (sd_device.h SLOT_FIRST) -------------------------------------------------------
+// A plan with FIRST / LAST declares NORDER > 0; only then do the loops below take the pair-aware paths, so every other plan's
+// kernel is the code it always was.
+template <class P, class = void> struct PlanOrders { static constexpr int N = 0; };
+template <class P> struct PlanOrders<P, decltype((void)P::NORDER)> { static constexpr int N = P::NORDER; };
+
+__device__ __forceinline__ bool order_wins(int op, uint64_t cand, uint64_t have) { return op == SLOT_FIRST ? cand < have : cand > have; }
+// pair (bk, bv) into (ak, av)
+__device__ __forceinline__ void order_combine(int op, uint64_t& ak, uint64_t& av, uint64_t bk, uint64_t bv) {
+  if (order_wins(op, bk, ak)) { ak = bk; av = bv; }
+}
+// 128-bit compare-and-swap of the pair at p (16-byte aligned): returns the pair found there
+template <bool SHARED>
+__device__ __forceinline__ void cas_pair(uint64_t* p, uint64_t ck, uint64_t cv, uint64_t nk, uint64_t nv, uint64_t& ok, uint64_t& ov) {
+  if (SHARED)
+    asm volatile("{\n\t.reg .b128 c, s, r;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 s, {%4, %5};\n\tatom.shared.cas.b128 r, [%6], c, s;\n\tmov.b128 {%0, %1}, r;\n\t}"
+                 : "=l"(ok), "=l"(ov) : "l"(ck), "l"(cv), "l"(nk), "l"(nv), "r"((uint32_t)__cvta_generic_to_shared(p)) : "memory");
+  else
+    asm volatile("{\n\t.reg .b128 c, s, r;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 s, {%4, %5};\n\tatom.global.cas.b128 r, [%6], c, s;\n\tmov.b128 {%0, %1}, r;\n\t}"
+                 : "=l"(ok), "=l"(ov) : "l"(ck), "l"(cv), "l"(nk), "l"(nv), "l"(p) : "memory");
+}
+// the pair at p (shared or global memory, by SHARED) takes (k, v) when k wins.  A plain load of the key first: rows that lose --
+// nearly every row of a FIRST -- issue no atomic.  The two words are read apart, so a CAS may fail on a torn expectation; it
+// returns the pair as it is and the loop decides again.
+template <bool SHARED>
+__device__ __forceinline__ void order_atomic(int op, uint64_t* p, uint64_t k, uint64_t v) {
+  uint64_t hk = *reinterpret_cast<volatile uint64_t*>(p);
+  if (!order_wins(op, k, hk)) return;
+  uint64_t hv = reinterpret_cast<volatile uint64_t*>(p)[1];
+  for (;;) {
+    uint64_t ok, ov;
+    cas_pair<SHARED>(p, hk, hv, k, v, ok, ov);
+    if (ok == hk && ov == hv) return;
+    hk = ok; hv = ov;
+    if (!order_wins(op, k, hk)) return;
+  }
+}
+// initial word of slot op of a plan (slot_identity, and the empty order keys of a plan with FIRST / LAST)
+template <class PLAN>
+__device__ __forceinline__ uint64_t slot_init(int op) {
+  if constexpr (PlanOrders<PLAN>::N > 0) return slot_initial(op);
+  else return slot_identity(op);
+}
+// sv into the NSLOT entries at a (entry s at a[s * stride]) without atomics
+template <class PLAN>
+__device__ __forceinline__ void combine_plain(uint64_t* a, int stride, const uint64_t* sv) {
+#pragma unroll
+  for (int s = 0; s < PLAN::NSLOT; s++) {
+    const int op = PLAN::slot_op(s);
+    if (is_order_op(op)) order_combine(op, a[s * stride], a[(s + 1) * stride], sv[s], sv[s + 1]);
+    else if (op != SLOT_PAIR_VAL) a[s * stride] = slot_combine(op, a[s * stride], sv[s]);
+  }
+}
+// sv into the NSLOT entries at t with atomics (shared or global memory, by SHARED)
+template <class PLAN, bool SHARED>
+__device__ __forceinline__ void combine_atomic(uint64_t* t, const uint64_t* sv) {
+#pragma unroll
+  for (int s = 0; s < PLAN::NSLOT; s++) {
+    const int op = PLAN::slot_op(s);
+    if (is_order_op(op)) order_atomic<SHARED>(op, t + s, sv[s], sv[s + 1]);
+    else if (op != SLOT_PAIR_VAL) slot_atomic(op, t + s, sv[s]);
+  }
+}
+
 // ---- MODE_HASH: find-or-insert of a key tuple, then atomic slot updates ---------------------------------
 __device__ __forceinline__ uint64_t hash_mix64(uint64_t h, uint64_t v) {
   h ^= v + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
@@ -1069,6 +1133,7 @@ struct RowCtx {
   uint64_t kpack[MAX_TABLES];
   const uint8_t* litpool;           // STRING literal bytes of this execution
   const uint8_t* strbase[64];       // per STRING scan column: body of an ENC_STR_RAW batch (refs are positions into it), else nullptr
+  uint64_t ord;                     // plans with FIRST / LAST: the current row's order key without its NULL flag
   __device__ __forceinline__ const uint8_t* table(int t) const { return tbl[t]; }
   __device__ __forceinline__ const uint8_t* lit_bytes(int slot) const { return litpool + (uint32_t)((uint64_t)L->i[slot] >> 32); }
   __device__ __forceinline__ int lit_len(int slot) const { return (int)((uint64_t)L->i[slot] & 0xffffffffull); }
@@ -1203,14 +1268,14 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
       for (int s = 0; s < NSLOT; s++) racc[gi][s] = slot_identity(PLAN::slot_op(s));
   } else if (PLAN::MODE == MODE_NOKEY) {
 #pragma unroll
-    for (int s = 0; s < NSLOT; s++) acc[s] = slot_identity(PLAN::slot_op(s));
+    for (int s = 0; s < NSLOT; s++) acc[s] = slot_init<PLAN>(PLAN::slot_op(s));
   } else if (PLAN::MODE == MODE_HASH || PLAN::MODE == MODE_PROJECT || PLAN::MODE == MODE_MUTATE) {
     // nothing per CTA: the table / output buffer is global
   } else if (args.table_mode == TABLE_PRIVATE) {
     // private table of thread t: entry e at table[e * THREADS + t]: lanes hit distinct banks
-    for (int e = 0; e < NE; e++) table[e * THREADS + tid] = slot_identity(PLAN::slot_op(e % NSLOT));
+    for (int e = 0; e < NE; e++) table[e * THREADS + tid] = slot_init<PLAN>(PLAN::slot_op(e % NSLOT));
   } else if (args.table_mode == TABLE_SHARED_ATOMIC) {
-    for (int e = tid; e < NE; e += THREADS) table[e] = slot_identity(PLAN::slot_op_rt(e % NSLOT));
+    for (int e = tid; e < NE; e += THREADS) table[e] = slot_init<PLAN>(PLAN::slot_op_rt(e % NSLOT));
     consumer_sync();
   }
   // moment aggregates: where a row finds its group's K (sd_device.h SHIFT_EMPTY).  The words beside the running result / hash
@@ -1218,6 +1283,8 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   // memory they fill on first touch
   constexpr int NSH = PlanShifts<PLAN>::N;
   static_assert(NSH == 0 || RG == 0, "the register-table variant is never built for plans with moment aggregates");
+  constexpr int NORD = PlanOrders<PLAN>::N;
+  static_assert(NORD == 0 || RG == 0, "the register-table variant is never built for plans with FIRST / LAST");
   uint64_t kreg[NSH > 0 ? NSH : 1];
   uint64_t* kcache = nullptr;
   (void)kreg; (void)kcache;
@@ -1378,6 +1445,8 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
         if (!PLAN::filter(row, ctx)) continue;      // FilterExec: only TRUE passes
         c_passed++;
         uint64_t sv[NSLOT > 0 ? NSLOT : 1];
+        if constexpr (NORD > 0)   // the row's order key (sd_device.h ORDER_EMPTY_FIRST) without its NULL flag
+          ctx.ord = ((uint64_t)(uint32_t)(args.batch_base + lo + 1) << 32) | ((uint64_t)(uint32_t)(tile_start + row_in_tile(r)) << 1);
         PLAN::slots(row, ctx, sv);
         if (PLAN::MODE == MODE_NOKEY) {
           if constexpr (NSH > 0)
@@ -1385,8 +1454,11 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
               if (kreg[i] == SHIFT_EMPTY) kreg[i] = shift_claim(args.shifts + i, c);
               return kreg[i];
             });
+          if constexpr (NORD > 0) combine_plain<PLAN>(acc, 1, sv);
+          else {
 #pragma unroll
-          for (int s = 0; s < NSLOT; s++) acc[s] = slot_combine(PLAN::slot_op(s), acc[s], sv[s]);
+            for (int s = 0; s < NSLOT; s++) acc[s] = slot_combine(PLAN::slot_op(s), acc[s], sv[s]);
+          }
         } else {
           if (PLAN::MODE == MODE_HASH) {
             int64_t kc[PLAN::NKEYS > 0 ? PLAN::NKEYS : 1];
@@ -1396,8 +1468,11 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
             if (e >= 0) {
               uint64_t* t = args.hash.vals + (size_t)e * NSLOT;
               if constexpr (NSH > 0) apply_shifts<PLAN>(sv, [&](int i, uint64_t c) { return shift_claim(args.hash.shifts + (size_t)e * NSH + i, c); });
+              if constexpr (NORD > 0) combine_atomic<PLAN, false>(t, sv);
+              else {
 #pragma unroll
-              for (int s = 0; s < NSLOT; s++) slot_atomic(PLAN::slot_op(s), t + s, sv[s]);
+                for (int s = 0; s < NSLOT; s++) slot_atomic(PLAN::slot_op(s), t + s, sv[s]);
+              }
             }
             continue;
           }
@@ -1423,8 +1498,14 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
             }
           } else if (args.table_mode == TABLE_PRIVATE) {
             uint64_t* t = table + (size_t)g * NSLOT * THREADS + tid;
+            if constexpr (NORD > 0) combine_plain<PLAN>(t, THREADS, sv);
+            else {
 #pragma unroll
-            for (int s = 0; s < NSLOT; s++) t[s * THREADS] = slot_combine(PLAN::slot_op(s), t[s * THREADS], sv[s]);
+              for (int s = 0; s < NSLOT; s++) t[s * THREADS] = slot_combine(PLAN::slot_op(s), t[s * THREADS], sv[s]);
+            }
+          } else if constexpr (NORD > 0) {
+            if (args.table_mode == TABLE_SHARED_ATOMIC) combine_atomic<PLAN, true>(table + (size_t)g * NSLOT, sv);
+            else combine_atomic<PLAN, false>(args.result + (size_t)g * NSLOT, sv);
           } else {
             uint64_t* t = (args.table_mode == TABLE_SHARED_ATOMIC ? table : args.result) + (size_t)g * NSLOT;
 #pragma unroll
@@ -1447,13 +1528,32 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     uint64_t* scratch = table;   // [NSLOT][THREADS/32]
 #pragma unroll
     for (int s = 0; s < NSLOT; s++) {
+      if constexpr (NORD > 0) {
+        const int op = PLAN::slot_op(s);
+        if (op == SLOT_PAIR_VAL) continue;
+        if (is_order_op(op)) {
+          uint64_t k = acc[s], v = acc[s + 1];
+#pragma unroll
+          for (int d = 16; d > 0; d >>= 1) order_combine(op, k, v, __shfl_xor_sync(0xffffffffu, k, d), __shfl_xor_sync(0xffffffffu, v, d));
+          if (lane == 0) { scratch[s * (THREADS / 32) + warp] = k; scratch[(s + 1) * (THREADS / 32) + warp] = v; }
+          continue;
+        }
+      }
       uint64_t v = acc[s];
 #pragma unroll
       for (int d = 16; d > 0; d >>= 1) v = slot_combine(PLAN::slot_op(s), v, __shfl_xor_sync(0xffffffffu, v, d));
       if (lane == 0) scratch[s * (THREADS / 32) + warp] = v;
     }
     consumer_sync();
-    if (tid < NSLOT) {
+    if (NORD > 0 && tid < NSLOT && is_order_op(PLAN::slot_op_rt(tid))) {
+      const int op = PLAN::slot_op_rt(tid);
+      uint64_t k = slot_initial(op), v = 0;
+      for (int w = 0; w < THREADS / 32; w++) order_combine(op, k, v, scratch[tid * (THREADS / 32) + w], scratch[(tid + 1) * (THREADS / 32) + w]);
+      my_partials[tid] = k;
+      my_partials[tid + 1] = v;
+    } else if (NORD > 0 && tid < NSLOT && PLAN::slot_op_rt(tid) == SLOT_PAIR_VAL) {
+      // written with its key
+    } else if (tid < NSLOT) {
       const int op = PLAN::slot_op_rt(tid);
       uint64_t v = slot_identity(op);
       for (int w = 0; w < THREADS / 32; w++) v = slot_combine(op, v, scratch[tid * (THREADS / 32) + w]);
@@ -1474,6 +1574,18 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     }
     for (int e = warp; e < NE; e += THREADS / 32) {
       const int op = PLAN::slot_op_rt(e % NSLOT);
+      if constexpr (NORD > 0) {
+        if (op == SLOT_PAIR_VAL) continue;
+        if (is_order_op(op)) {
+          uint64_t k = slot_initial(op), v = 0;
+#pragma unroll
+          for (int j = 0; j < THREADS / 32; j++) order_combine(op, k, v, table[e * THREADS + lane + 32 * j], table[(e + 1) * THREADS + lane + 32 * j]);
+#pragma unroll
+          for (int d = 16; d > 0; d >>= 1) order_combine(op, k, v, __shfl_xor_sync(0xffffffffu, k, d), __shfl_xor_sync(0xffffffffu, v, d));
+          if (lane == 0) { my_partials[e] = k; my_partials[e + 1] = v; }
+          continue;
+        }
+      }
       uint64_t v = slot_identity(op);
 #pragma unroll
       for (int j = 0; j < THREADS / 32; j++) v = slot_combine(op, v, table[e * THREADS + lane + 32 * j]);
@@ -1500,6 +1612,18 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     __threadfence();
     for (int e = tid; e < NE; e += THREADS) {
       const int op = PLAN::slot_op_rt(e % NSLOT);
+      if constexpr (NORD > 0) {
+        if (op == SLOT_PAIR_VAL) continue;
+        if (is_order_op(op)) {
+          uint64_t k = slot_initial(op), v = 0;
+          for (unsigned bk = 0; bk < gridDim.x; bk++)
+            order_combine(op, k, v, __ldcg(&args.partials[(size_t)bk * NE + e]), __ldcg(&args.partials[(size_t)bk * NE + e + 1]));
+          if (!args.fresh) { uint64_t rk = args.result[e], rv = args.result[e + 1]; order_combine(op, rk, rv, k, v); k = rk; v = rv; }
+          args.result[e] = k;
+          args.result[e + 1] = v;
+          continue;
+        }
+      }
       uint64_t v = slot_identity(op);
       for (unsigned bk = 0; bk < gridDim.x; bk++) v = slot_combine(op, v, __ldcg(&args.partials[(size_t)bk * NE + e]));
       args.result[e] = args.fresh ? v : slot_combine(op, args.result[e], v);

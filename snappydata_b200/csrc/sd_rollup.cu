@@ -3,7 +3,8 @@
 //
 // Spark plans these queries as Expand (every row once per set, absent keys NULL, spark_grouping_id appended) under the partial
 // aggregate.  Every set is a coarsening of the grouping by all n keys and every slot of the scan is decomposable (slot_atomic
-// combines it; moment and covariance sums are re-centred on the coarse group's shift), so the device scans once with the plan's
+// combines it; moment and covariance sums are re-centred on the coarse group's shift; a FIRST / LAST pair keeps the fine group
+// whose order key wins), so the device scans once with the plan's
 // plain kernel and this kernel combines each (fine group, set) into a hash table keyed by (k1..kn with absent keys NULL, gid):
 // work proportional to groups x sets, not to rows.
 #include <algorithm>
@@ -81,7 +82,9 @@ __global__ void rollup_kernel(RollupArgs a) {
         const double n = (double)sv[a.shift_count[ix]], Sx = u2f(sv[a.shift_pow[ix * 4]]), Sy = u2f(sv[a.shift_pow[iy * 4]]);
         v = f2u(u2f(v) + dy * Sx + dx * Sy + n * dx * dy);
       }
-      slot_atomic(a.slot_op[s], cv + s, v);
+      const int op = a.slot_op[s];
+      if (is_order_op(op)) { order_atomic<false>(op, cv + s, v, sv[s + 1]); s++; continue; }   // FIRST / LAST: the fine group's pair
+      slot_atomic(op, cv + s, v);
     }
   }
 }

@@ -143,6 +143,9 @@ class PlanBuilder:
     def covar_pop(self, x: E, y: E): return self.agg(AggFn.COVAR_POP, self.pair(x, y))
     def covar_samp(self, x: E, y: E): return self.agg(AggFn.COVAR_SAMP, self.pair(x, y))
     def corr(self, x: E, y: E): return self.agg(AggFn.CORR, self.pair(x, y))
+    # Spark's first / first_value and last / last_value: the value of the first / last row in scan order
+    def first(self, e: E, ignore_nulls: bool = False): return self.agg(AggFn.FIRST_IGNORE_NULLS if ignore_nulls else AggFn.FIRST, e)
+    def last(self, e: E, ignore_nulls: bool = False): return self.agg(AggFn.LAST_IGNORE_NULLS if ignore_nulls else AggFn.LAST, e)
     def project(self, *es: E): self._proj = list(es); return self
 
     # UPDATE / DELETE over a resident store (SD_PLAN_MUTATE; the WHERE clause is filter())
