@@ -36,31 +36,6 @@ bool node_is_wide(const PlanSpec& p, int node) {
 }
 int kind_of_column(const sd_column& c) { return wide_decimal(c.type, c.precision) ? K_CODE : kind_of_type(c.type); }
 static const char* col_ctype(const sd_column& c);
-std::vector<int> partial_field_types(const PlanSpec& p) {
-  std::vector<int> t;
-  for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
-  if (p.gid_node >= 0) t.push_back(SD_INT);   // spark_grouping_id
-  for (auto& m : p.agg_map) {
-    if (is_moment(m.fn) || is_pair_agg(m.fn)) { t.insert(t.end(), (size_t)agg_buffer_fields(m.fn), SD_DOUBLE); continue; }
-    t.push_back(field_type(m.buf_type, m.buf_ps)); if (m.fn == SD_AGG_AVG) t.push_back(SD_LONG);
-    if (is_order_agg(m.fn)) t.push_back(SD_BOOLEAN);   // valueSet
-  }
-  return t;
-}
-std::vector<int> final_field_types(const PlanSpec& p) {
-  std::vector<int> t;
-  for (int k : p.keys) t.push_back(field_type(p.exprs[k].type, p.exprs[k].type == SD_DECIMAL ? decimal_ps(p, k) : 0));
-  if (p.gid_node >= 0) t.push_back(SD_INT);
-  for (auto& m : p.agg_map) {
-    if (m.fn == SD_AGG_AVG) {
-      if (m.buf_type == SD_DECIMAL) {   // Average.resultType: DecimalType.bounded(p + 4, s + 4)
-        const int pr = std::min(38, (m.in_ps >> 8) + 4), sc = std::min(38, (m.in_ps & 0xff) + 4);
-        t.push_back(field_type(SD_DECIMAL, (pr << 8) | sc));
-      } else t.push_back(SD_DOUBLE);
-    } else t.push_back(field_type(m.buf_type, m.buf_ps));
-  }
-  return t;
-}
 
 int kind_of_type(int t) {
   switch (t) {
@@ -110,6 +85,12 @@ static bool is_unary(int op) {
 }
 static bool is_cmp(int op) { return op >= SD_OP_EQ && op <= SD_OP_GE; }
 static bool is_grouping_node(int op) { return op == SD_OP_GROUPING_SET || op == SD_OP_GROUPING_ID; }
+// AggFamily of an SD_AGG_* code (1..19), -1 when unknown
+static int agg_family(int fn) {
+  static const int family[] = {-1, AGG_COUNT, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MINMAX, AGG_MINMAX, AGG_MOMENT, AGG_MOMENT, AGG_MOMENT,
+                               AGG_MOMENT, AGG_MOMENT, AGG_MOMENT, AGG_PAIR, AGG_PAIR, AGG_PAIR, AGG_ORDER, AGG_ORDER, AGG_ORDER, AGG_ORDER};
+  return fn >= 1 && fn <= SD_AGG_LAST_IGNORE_NULLS ? family[fn] : -1;
+}
 
 sd_plan_desc PlanSpec::desc_view() const {
   sd_plan_desc d;
@@ -155,7 +136,7 @@ static bool string_predicate_col(const PlanSpec& p, int node, int* col) {
   return false;
 }
 
-static int cmp_bytes(const char* a, int la, const char* b, int lb) {
+int cmp_bytes(const char* a, int la, const char* b, int lb) {
   int n = la < lb ? la : lb;
   int c = n ? memcmp(a, b, n) : 0;
   return c ? c : la - lb;
@@ -323,8 +304,9 @@ struct Gen {
     for (int k : p.keys) if (is_pair(k)) return fail(SD_ERR_INVALID, "a PAIR node cannot be a grouping key");
     for (int k : p.proj) if (is_pair(k)) return fail(SD_ERR_INVALID, "a PAIR node cannot be projected or assigned");
     for (auto& a : p.aggs) {
-      if (is_pair_agg(a.fn) && (a.expr < 0 || !is_pair(a.expr))) return fail(SD_ERR_INVALID, "COVAR_POP / COVAR_SAMP / CORR need a PAIR node input");
-      if (!is_pair_agg(a.fn) && a.expr >= 0 && is_pair(a.expr)) return fail(SD_ERR_INVALID, "a PAIR node is only the input of COVAR_POP / COVAR_SAMP / CORR");
+      const bool pair_agg = agg_family(a.fn) == AGG_PAIR;
+      if (pair_agg && (a.expr < 0 || !is_pair(a.expr))) return fail(SD_ERR_INVALID, "COVAR_POP / COVAR_SAMP / CORR need a PAIR node input");
+      if (!pair_agg && a.expr >= 0 && is_pair(a.expr)) return fail(SD_ERR_INVALID, "a PAIR node is only the input of COVAR_POP / COVAR_SAMP / CORR");
     }
     return 0;
   }
@@ -378,24 +360,39 @@ struct Gen {
     return add_slot(SLOT_ADD_I64, node, GATE_NONNULL_COUNT);
   }
 
+  // the buffer of SUM / MIN / MAX is nullable when its input is (grouped: SnappyHashAggregateExec.scala:174-210) and always
+  // without keys (a plain Spark buffer, NULL until the first non-null input, :337-346); a nullable buffer counts its inputs
+  void nullable_buffer(AggMap& m, int node, bool keyed) {
+    m.buf_nullable = keyed ? static_nullable(node) : 1;
+    if (m.buf_nullable) m.count_slot = count_slot_for(node);
+  }
+  // the STRING column's TABLE_KEYPTR table that aggregates share, added on first use
+  int keyptr_table(int col) {
+    for (size_t t = 0; t < p.tables.size(); t++)
+      if (p.tables[t].kind == TABLE_KEYPTR && p.tables[t].col == col && p.tables[t].key < 0) return (int)t;
+    p.tables.push_back(TableSpec{TABLE_KEYPTR, col, -1, -1});
+    return (int)p.tables.size() - 1;
+  }
+
   int build_slots() {
     const bool keyed = !p.keys.empty();
     for (auto& a : p.aggs) {
       AggMap m;
       memset(&m, 0, sizeof(m));
-      m.fn = a.fn; m.value_slot = -1; m.count_slot = -1; m.shift = -1; m.shift_y = -1; m.order_slot = -1;
+      m.fn = a.fn; m.family = agg_family(a.fn); m.hold = HOLD_WORD;
+      m.value_slot = -1; m.value_slot2 = -1; m.count_slot = -1; m.shift = -1; m.shift_y = -1; m.order_slot = -1;
       for (int& l : m.limb_slot) l = -1;
       for (int& s : m.pow_slot) s = -1;
       for (int& s : m.pair_slot) s = -1;
       const int it = a.expr >= 0 ? p.exprs[a.expr].type : SD_LONG;
-      const int in_null = a.expr >= 0 ? static_nullable(a.expr) : 0;
-      m.in_type = it;
       if (a.fn != SD_AGG_COUNT_STAR && a.expr < 0) return fail(SD_ERR_INVALID, "aggregate without input expression");
-      if (is_moment(a.fn)) {
+      if (it == SD_DECIMAL) m.buf_ps = m.in_ps = decimal_ps(p, a.expr);   // MIN / MAX / FIRST / LAST keep the input type
+      const bool wide = a.expr >= 0 && node_is_wide(p, a.expr);
+      if (m.family == AGG_MOMENT) {
         // n = the non-null count, S_j = sum (x - K)^j around the group's shift K; the host turns them into Spark's buffers
         if (it != SD_DOUBLE) return fail(SD_ERR_INVALID, "STDDEV / VARIANCE / SKEWNESS / KURTOSIS need a DOUBLE input (cast it)");
         m.buf_type = SD_DOUBLE;
-        m.value_slot2 = -1;
+        m.hold = HOLD_SHIFTED;
         m.count_slot = count_slot_for(a.expr);
         const int order = moment_order(a.fn);
         for (int j = 0; j < order; j++) m.pow_slot[j] = add_slot(SLOT_ADD_F64, a.expr, GATE_POW1 + j);
@@ -408,11 +405,11 @@ struct Gen {
         p.agg_map.push_back(m);
         continue;
       }
-      if (is_pair_agg(a.fn)) {
+      if (m.family == AGG_PAIR) {
         // n = the count of rows with x and y non-null; S_x, S_y, S_xy (+ CORR's S_xx, S_yy) around the group's (Kx, Ky)
         const bool corr = a.fn == SD_AGG_CORR;
         m.buf_type = SD_DOUBLE;
-        m.value_slot2 = -1;
+        m.hold = HOLD_SHIFTED;
         m.count_slot = count_slot_for(a.expr);   // the PAIR node is NULL when x or y is
         for (int j = 0; j < (corr ? 5 : 3); j++) m.pair_slot[j] = add_slot(SLOT_ADD_F64, a.expr, GATE_PAIR_X + j);
         m.value_slot = m.pair_slot[2];
@@ -435,17 +432,16 @@ struct Gen {
         p.agg_map.push_back(m);
         continue;
       }
-      if (is_order_agg(a.fn)) {
+      if (m.family == AGG_ORDER) {
         // one (order key, value) pair at an even slot index; FIRST and LAST of one input, or one function with and without
         // ignoreNulls, keep pairs of their own
-        const bool str = it == SD_STRING, wide = node_is_wide(p, a.expr);
+        const bool str = it == SD_STRING;
         if ((str || wide) && p.exprs[a.expr].op != SD_OP_COL)
           return fail(SD_ERR_UNSUPPORTED, "FIRST / LAST of a STRING or wide DECIMAL expression that is not a column");
         m.buf_type = it;
+        m.hold = str || wide ? HOLD_REF : HOLD_WORD;
         m.buf_nullable = 1;
-        m.value_slot2 = -1;
-        if (it == SD_DECIMAL) { m.in_ps = decimal_ps(p, a.expr); m.buf_ps = m.in_ps; }
-        const int op = is_last_agg(a.fn) ? SLOT_LAST : SLOT_FIRST;
+        const int op = a.fn == SD_AGG_LAST || a.fn == SD_AGG_LAST_IGNORE_NULLS ? SLOT_LAST : SLOT_FIRST;
         const int gate = a.fn == SD_AGG_FIRST_IGNORE_NULLS || a.fn == SD_AGG_LAST_IGNORE_NULLS ? GATE_ORDER_KEY_IGN : GATE_ORDER_KEY;
         const std::string in = expr_text(p, a.expr);
         for (size_t q = 0; q < p.slots.size(); q++)
@@ -455,99 +451,48 @@ struct Gen {
           m.order_slot = (int)p.slots.size();
           p.slots.push_back(SlotSpec{op, a.expr, gate});
           p.slots.push_back(SlotSpec{SLOT_PAIR_VAL, a.expr, GATE_ORDER_VAL});
-          if (str) {   // the value is the address of the row's record, as for MIN / MAX over STRING
-            const int col = p.exprs[a.expr].a;
-            int t = -1;
-            for (size_t ti = 0; ti < p.tables.size(); ti++) if (p.tables[ti].kind == TABLE_KEYPTR && p.tables[ti].col == col && p.tables[ti].key < 0) t = (int)ti;
-            if (t < 0) { p.tables.push_back(TableSpec{TABLE_KEYPTR, col, -1, -1}); t = (int)p.tables.size() - 1; }
-            p.slots.back().table = t;
-          }
+          // a STRING value is the address of the row's record, as for MIN / MAX over STRING
+          if (str) p.slots.back().table = keyptr_table(p.exprs[a.expr].a);
           p.norder++;
         }
         m.value_slot = m.order_slot + 1;
         p.agg_map.push_back(m);
         continue;
       }
-      if (a.expr >= 0 && it == SD_STRING && a.fn != SD_AGG_COUNT) {
-        // MIN / MAX over a STRING column: the slot holds the address of the winning value's record (compared by bytes)
-        if (!(a.fn == SD_AGG_MIN || a.fn == SD_AGG_MAX) || p.exprs[a.expr].op != SD_OP_COL)
-          return fail(SD_ERR_UNSUPPORTED, "aggregates over STRING: only MIN / MAX / COUNT of a STRING column");
-        m.buf_type = SD_STRING;
-        m.value_slot2 = -1;
-        const int col = p.exprs[a.expr].a;
-        int t = -1;
-        for (size_t ti = 0; ti < p.tables.size(); ti++) if (p.tables[ti].kind == TABLE_KEYPTR && p.tables[ti].col == col && p.tables[ti].key < 0) t = (int)ti;
-        if (t < 0) { p.tables.push_back(TableSpec{TABLE_KEYPTR, col, -1, -1}); t = (int)p.tables.size() - 1; }
-        m.value_slot = add_slot(a.fn == SD_AGG_MIN ? SLOT_MIN_STR : SLOT_MAX_STR, a.expr, GATE_STRREF);
-        p.slots[m.value_slot].table = t;
-        m.buf_nullable = keyed ? in_null : 1;
-        if (m.buf_nullable) m.count_slot = count_slot_for(a.expr);
-        p.agg_map.push_back(m);
-        continue;
-      }
-      m.value_slot2 = -1;
-      if (it == SD_DECIMAL) {
-        m.in_ps = decimal_ps(p, a.expr);
-        m.buf_ps = m.in_ps;   // MIN / MAX keep the input type
-      }
-      if ((a.fn == SD_AGG_MIN || a.fn == SD_AGG_MAX) && node_is_wide(p, a.expr)) {
-        // the slot holds the address of the winning value's record, compared by value
-        if (p.exprs[a.expr].op != SD_OP_COL) return fail(SD_ERR_UNSUPPORTED, "MIN / MAX of a wide DECIMAL expression that is not a column");
-        m.buf_type = SD_DECIMAL;
-        m.value_slot = add_slot(a.fn == SD_AGG_MIN ? SLOT_MIN_DEC : SLOT_MAX_DEC, a.expr, GATE_DECREF);
-        m.buf_nullable = keyed ? in_null : 1;
-        if (m.buf_nullable) m.count_slot = count_slot_for(a.expr);
-        p.agg_map.push_back(m);
-        continue;
-      }
-      if ((a.fn == SD_AGG_SUM || a.fn == SD_AGG_AVG) && node_is_wide(p, a.expr)) {
-        // buffer DECIMAL(min(38, p + 10), s); the value is summed as four 32-bit limbs, recombined on the host
-        m.buf_type = SD_DECIMAL;
-        m.buf_ps = (std::min(38, (m.in_ps >> 8) + 10) << 8) | (m.in_ps & 0xff);
-        for (int l = 0; l < 4; l++) m.limb_slot[l] = add_slot(SLOT_ADD_I64, a.expr, GATE_LIMB0 + l);
-        m.value_slot = m.limb_slot[3];
-        if (a.fn == SD_AGG_SUM) { m.buf_nullable = keyed ? in_null : 1; if (m.buf_nullable) m.count_slot = count_slot_for(a.expr); }
-        else m.count_slot = count_slot_for(a.expr);
-        p.agg_map.push_back(m);
-        continue;
-      }
-      if ((a.fn == SD_AGG_SUM || a.fn == SD_AGG_AVG) && it == SD_DECIMAL) {
-        // Spark 2.1.1 Sum / Average over DECIMAL(p,s): buffer DECIMAL(p+10,s) -- up to 28 digits, i.e. wider than int64.
-        // The value is summed as two int64 slots (high / low 32 bits), exact for < 2^31 rows, and recombined on the host.
-        m.buf_type = SD_DECIMAL;
-        m.buf_ps = (std::min(38, (m.in_ps >> 8) + 10) << 8) | (m.in_ps & 0xff);
-        m.value_slot = add_slot(SLOT_ADD_I64, a.expr, GATE_VALUE_HI32);
-        m.value_slot2 = add_slot(SLOT_ADD_I64, a.expr, GATE_VALUE_LO32);
-        if (a.fn == SD_AGG_SUM) { m.buf_nullable = keyed ? in_null : 1; if (m.buf_nullable) m.count_slot = count_slot_for(a.expr); }
-        else m.count_slot = count_slot_for(a.expr);
-        p.agg_map.push_back(m);
-        continue;
-      }
-      switch (a.fn) {
-        case SD_AGG_COUNT_STAR:
-          m.value_slot = add_slot(SLOT_ADD_I64, -1, GATE_ONE); m.buf_type = SD_LONG; break;
-        case SD_AGG_COUNT:
-          m.value_slot = count_slot_for(a.expr); m.buf_type = SD_LONG; break;
-        case SD_AGG_SUM:
-          m.buf_type = sum_buffer_type(it);
-          m.value_slot = add_slot(m.buf_type == SD_DOUBLE ? SLOT_ADD_F64 : SLOT_ADD_I64, a.expr, GATE_VALUE);
-          // grouped: buffer non-nullable when the child is (SnappyHashAggregateExec.scala:174-210);
-          // no keys: plain Spark buffer, NULL until the first non-null input (:337-346)
-          m.buf_nullable = keyed ? in_null : 1;
-          if (m.buf_nullable) m.count_slot = count_slot_for(a.expr);
+      if (a.expr >= 0 && it == SD_STRING && a.fn != SD_AGG_COUNT && (m.family != AGG_MINMAX || p.exprs[a.expr].op != SD_OP_COL))
+        return fail(SD_ERR_UNSUPPORTED, "aggregates over STRING: only MIN / MAX / COUNT of a STRING column");
+      switch (m.family) {
+        case AGG_COUNT:
+          m.value_slot = a.fn == SD_AGG_COUNT_STAR ? add_slot(SLOT_ADD_I64, -1, GATE_ONE) : count_slot_for(a.expr);
+          m.buf_type = SD_LONG;
           break;
-        case SD_AGG_AVG:
-          m.buf_type = SD_DOUBLE;
-          m.value_slot = add_slot(SLOT_ADD_F64, a.expr, GATE_VALUE);
-          m.count_slot = count_slot_for(a.expr);
+        case AGG_SUM: case AGG_AVG:
+          if (it == SD_DECIMAL) {
+            // Spark 2.1.1 Sum / Average over DECIMAL(p,s): buffer DECIMAL(min(38, p + 10), s) -- up to 28 digits from an input
+            // of at most 18, i.e. wider than int64, so the value is summed in 32-bit parts (exact for < 2^31 rows) recombined on
+            // the host: four limbs of a wide input, else the high / low halves
+            m.buf_type = SD_DECIMAL;
+            m.buf_ps = (std::min(38, (m.in_ps >> 8) + 10) << 8) | (m.in_ps & 0xff);
+            m.hold = wide ? HOLD_LIMBS : HOLD_HILO;
+            if (wide) for (int l = 0; l < 4; l++) m.value_slot = m.limb_slot[l] = add_slot(SLOT_ADD_I64, a.expr, GATE_LIMB0 + l);
+            else { m.value_slot = add_slot(SLOT_ADD_I64, a.expr, GATE_VALUE_HI32); m.value_slot2 = add_slot(SLOT_ADD_I64, a.expr, GATE_VALUE_LO32); }
+          } else {
+            m.buf_type = m.family == AGG_AVG ? SD_DOUBLE : sum_buffer_type(it);
+            m.value_slot = add_slot(m.buf_type == SD_DOUBLE ? SLOT_ADD_F64 : SLOT_ADD_I64, a.expr, GATE_VALUE);
+          }
+          if (m.family == AGG_SUM) nullable_buffer(m, a.expr, keyed);
+          else m.count_slot = count_slot_for(a.expr);
           break;
-        case SD_AGG_MIN: case SD_AGG_MAX: {
+        case AGG_MINMAX: {
+          const bool str = it == SD_STRING, fp = type_is_fp(it), min = a.fn == SD_AGG_MIN;
           m.buf_type = it;
-          const bool fp = type_is_fp(it);
-          const int op = a.fn == SD_AGG_MIN ? (fp ? SLOT_MIN_F64 : SLOT_MIN_I64) : (fp ? SLOT_MAX_F64 : SLOT_MAX_I64);
-          m.value_slot = add_slot(op, a.expr, GATE_VALUE);
-          m.buf_nullable = keyed ? in_null : 1;
-          if (m.buf_nullable) m.count_slot = count_slot_for(a.expr);
+          if (str || wide) {   // the slot holds the address of the winning value's record, compared by bytes (STRING) or by value
+            if (p.exprs[a.expr].op != SD_OP_COL) return fail(SD_ERR_UNSUPPORTED, "MIN / MAX of a wide DECIMAL expression that is not a column");
+            m.hold = HOLD_REF;
+            m.value_slot = add_slot(str ? (min ? SLOT_MIN_STR : SLOT_MAX_STR) : (min ? SLOT_MIN_DEC : SLOT_MAX_DEC), a.expr, str ? GATE_STRREF : GATE_DECREF);
+            if (str) p.slots[m.value_slot].table = keyptr_table(p.exprs[a.expr].a);
+          } else m.value_slot = add_slot(min ? (fp ? SLOT_MIN_F64 : SLOT_MIN_I64) : (fp ? SLOT_MAX_F64 : SLOT_MAX_I64), a.expr, GATE_VALUE);
+          nullable_buffer(m, a.expr, keyed);
           break;
         }
         default: return fail(SD_ERR_INVALID, "unknown aggregate function");

@@ -49,18 +49,30 @@ struct SlotSpec {
   int table = -1;   // GATE_STRREF: index of the column's TABLE_KEYPTR table
 };
 
+// An aggregate's function family (Spark's buffers have one shape per family; MIN vs MAX, FIRST vs LAST and ignoreNulls are
+// read from AggMap.fn), and how its slots carry the first buffer value:
+//   HOLD_WORD    one slot word, int64 or the double's bits by buf_type
+//   HOLD_HILO    DECIMAL SUM / AVG: the high and low 32-bit halves summed in value_slot / value_slot2
+//   HOLD_LIMBS   wide DECIMAL SUM / AVG: four 32-bit limbs summed in limb_slot[0..3]
+//   HOLD_REF     the device address of the value's [len][bytes] record (STRING, DECIMAL wider than 18 digits)
+//   HOLD_SHIFTED moment / two-input sums around the group's K words
+// build_slots (sd_codegen.cpp) decides both; sd_aggregate.cpp turns slots into Spark's buffers by them
+enum AggFamily { AGG_COUNT = 0, AGG_SUM = 1, AGG_AVG = 2, AGG_MINMAX = 3, AGG_MOMENT = 4, AGG_PAIR = 5, AGG_ORDER = 6 };
+enum AggHold { HOLD_WORD = 0, HOLD_HILO = 1, HOLD_LIMBS = 2, HOLD_REF = 3, HOLD_SHIFTED = 4 };
+
 // how an aggregate's buffer fields map to slots
 struct AggMap {
   int fn;
+  int family;       // AggFamily
+  int hold;         // AggHold
   int value_slot;   // SUM/AVG sum, MIN/MAX value, COUNT count
   int count_slot;   // AVG count; SUM/MIN/MAX non-null count when the buffer is nullable (-1 otherwise)
-  int in_type;      // sd_type of the input
   int buf_type;     // sd_type of the (first) buffer field
   int buf_nullable;
-  int value_slot2;  // DECIMAL SUM/AVG: the low-half slot (value_slot holds the high half); -1 otherwise
+  int value_slot2;  // HOLD_HILO: the low-half slot (value_slot holds the high half); -1 otherwise
   int in_ps;        // DECIMAL input: (precision << 8) | scale; 0 otherwise
   int buf_ps;       // DECIMAL buffer: SUM/AVG (p + 10, s) bounded to 38; MIN/MAX = input
-  int limb_slot[4]; // SUM/AVG of a wide DECIMAL: the slots of limbs 0..3 (value_slot = limb 3, value_slot2 = -1); else -1
+  int limb_slot[4]; // HOLD_LIMBS: the slots of limbs 0..3 (value_slot = limb 3); else -1
   int shift;        // moment aggregate: index of its input's shift in PlanSpec.shifts (count_slot = n, value_slot = S_1); else -1
   int pow_slot[4];  // moment aggregate: S_1..S_order; else -1
   int shift_y;      // two-input aggregate: index of its y shift (`shift` is the x shift; count_slot = n, value_slot = S_xy); else -1
@@ -68,19 +80,8 @@ struct AggMap {
   int order_slot;   // FIRST / LAST: the pair's key slot (value_slot = order_slot + 1 holds the value); else -1
 };
 
-// a moment aggregate (Spark 2.1.1 CentralMomentAgg): STDDEV_* / VAR_* (order 2), SKEWNESS (3), KURTOSIS (4)
-inline bool is_moment(int fn) { return fn >= SD_AGG_STDDEV_POP && fn <= SD_AGG_KURTOSIS; }
+// a moment aggregate's highest power: STDDEV_* / VAR_* 2, SKEWNESS 3, KURTOSIS 4
 inline int moment_order(int fn) { return fn == SD_AGG_KURTOSIS ? 4 : fn == SD_AGG_SKEWNESS ? 3 : 2; }
-// a two-input aggregate (Spark 2.1.1 Covariance / Corr) over an SD_OP_PAIR node
-inline bool is_pair_agg(int fn) { return fn >= SD_AGG_COVAR_POP && fn <= SD_AGG_CORR; }
-// FIRST / LAST with or without ignoreNulls (Spark 2.1.1 First / Last)
-inline bool is_order_agg(int fn) { return fn >= SD_AGG_FIRST && fn <= SD_AGG_LAST_IGNORE_NULLS; }
-inline bool is_last_agg(int fn) { return fn == SD_AGG_LAST || fn == SD_AGG_LAST_IGNORE_NULLS; }
-// partial-row buffer fields of an aggregate: AVG [sum, count]; moments [n, avg, m2, (m3, (m4))]; COVAR_* [n, xAvg, yAvg, ck];
-// CORR [n, xAvg, yAvg, ck, xMk, yMk]; FIRST / LAST [value, valueSet]; others one
-inline int agg_buffer_fields(int fn) {
-  return fn == SD_AGG_AVG || is_order_agg(fn) ? 2 : is_moment(fn) ? 1 + moment_order(fn) : fn == SD_AGG_CORR ? 6 : is_pair_agg(fn) ? 4 : 1;
-}
 
 // one shift K of a plan's moment sums (its K words are not slots, sd_device.h SHIFT_EMPTY): every moment aggregate over the
 // same input shares it and its S_j slots
@@ -159,13 +160,12 @@ int analyze_plan(const sd_plan_desc* desc, PlanSpec& out, std::string& err, cons
 // Host evaluation of a string predicate node for one dictionary entry (used to fill truth tables):
 // returns 0 FALSE, 1 TRUE, 2 NULL.  `s == nullptr` means the NULL code.
 int eval_string_predicate(const PlanSpec& p, int node, const char* s, int slen, const sd_literal* lits);
+// byte-wise comparison of two strings: < 0, 0, > 0
+int cmp_bytes(const char* a, int la, const char* b, int lb);
 
 int sum_buffer_type(int t);
 // (precision << 8) | scale of a DECIMAL-typed expression node
 int decimal_ps(const PlanSpec& p, int node);
-// partial-row field types (keys ++ aggregate buffers) and final-row field types (keys ++ results) as field_type codes
-std::vector<int> partial_field_types(const PlanSpec& p);
-std::vector<int> final_field_types(const PlanSpec& p);
 bool type_is_integral(int t);
 bool type_is_fp(int t);
 int kind_of_type(int t);

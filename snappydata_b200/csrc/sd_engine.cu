@@ -1,9 +1,7 @@
 // sd_engine.cu -- plan handles: stats-row batch skipping, per-batch descriptor/table preparation,
-// kernel launch, partial-row emission, final merge.  Host-side counterpart of
+// kernel launch, partial-row emission (the buffers themselves: sd_aggregate.cpp).  Host-side counterpart of
 //   ColumnTableScan.doProduce batch loop        core/execution/columnar/ColumnTableScan.scala:518-599
 //   ColumnTableScan.generateStatPredicate       core/execution/columnar/ColumnTableScan.scala:820-963
-//   SnappyHashAggregateExec partial output      core/execution/aggregate/SnappyHashAggregateExec.scala:1148-1178
-//   CollectAggregateExec / final merge          core/execution/aggregate/CollectAggregateExec.scala:67-121
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -12,6 +10,7 @@
 #include <map>
 #include <mutex>
 
+#include "sd_aggregate.h"
 #include "sd_host.h"
 
 using namespace sd;
@@ -19,147 +18,6 @@ using namespace sd;
 namespace {
 
 thread_local int t_device = 0;
-
-inline int32_t rd_i32(const uint8_t* p) { int32_t v; memcpy(&v, p, 4); return v; }
-inline int16_t rd_i16(const uint8_t* p) { int16_t v; memcpy(&v, p, 2); return v; }
-inline int64_t rd_i64(const uint8_t* p) { int64_t v; memcpy(&v, p, 8); return v; }
-inline double rd_f64(const uint8_t* p) { double v; memcpy(&v, p, 8); return v; }
-inline float rd_f32(const uint8_t* p) { float v; memcpy(&v, p, 4); return v; }
-
-// ---- host values (stats rows, partial rows) -------------------------------------------------------
-typedef __int128 i128;
-struct HVal {
-  bool isnull = false;
-  int64_t i = 0;
-  double d = 0;
-  i128 w = 0;      // DECIMAL unscaled value (any precision); `i` mirrors it when the precision is <= 18
-  // merge of wide-DECIMAL SUM / AVG buffers (wide_acc_add): the exact total as acc_hi * 2^64 + acc_lo, and whether an input
-  // had already overflowed
-  unsigned __int128 acc_lo = 0;
-  i128 acc_hi = 0;
-  bool acc = false, ovf = false;
-  std::string s;
-};
-i128 pow10_128(int k) { i128 r = 1; for (int j = 0; j < k; j++) r *= 10; return r; }
-// BigInteger(bytes): big-endian two's complement, 1..16 bytes (a wide DECIMAL record's or literal's unscaled value)
-i128 dec_from_bytes(const uint8_t* b, size_t n) {
-  unsigned __int128 u = (unsigned __int128)(i128)(int8_t)b[0];
-  for (size_t k = 1; k < n; k++) u = (u << 8) | b[k];
-  return (i128)u;
-}
-
-int cmp_str(const std::string& a, const std::string& b) {
-  size_t n = std::min(a.size(), b.size());
-  int c = n ? memcmp(a.data(), b.data(), n) : 0;
-  return c ? c : (a.size() < b.size() ? -1 : (a.size() > b.size() ? 1 : 0));
-}
-int cmp_f64(double x, double y) {   // Utils.nanSafeCompareDoubles
-  const bool xn = std::isnan(x), yn = std::isnan(y);
-  if (xn || yn) return xn && yn ? 0 : (xn ? 1 : -1);
-  return x < y ? -1 : (x > y ? 1 : 0);
-}
-int cmp_hval(const HVal& a, const HVal& b, int ft) {
-  const int t = ft_base(ft);
-  if (t == SD_STRING) return cmp_str(a.s, b.s);
-  if (type_is_fp(t)) return cmp_f64(a.d, b.d);
-  if (t == SD_DECIMAL) return a.w < b.w ? -1 : (a.w > b.w ? 1 : 0);
-  return a.i < b.i ? -1 : (a.i > b.i ? 1 : 0);
-}
-
-// field `idx` of a Spark UnsafeRow with `nfields` fields (SURVEY.md Appendix B.9)
-bool unsafe_field(const uint8_t* row, int64_t len, int nfields, int idx, int ftype, HVal* out) {
-  const int64_t bits = ((nfields + 63) / 64) * 8;
-  if (idx < 0 || idx >= nfields || bits + 8 * (int64_t)nfields > len) return false;
-  *out = HVal();
-  if (row[idx >> 3] & (1u << (idx & 7))) { out->isnull = true; return true; }
-  const uint8_t* slot = row + bits + 8 * (int64_t)idx;
-  const int type = ft_base(ftype);
-  if (type == SD_DECIMAL) {   // UnsafeRow.getDecimal: long for precision <= 18, else BigInteger bytes (big-endian two's complement)
-    if (ft_precision(ftype) <= 18) { out->i = rd_i64(slot); out->w = out->i; return true; }
-    const int64_t ol = rd_i64(slot);
-    const int64_t off = ol >> 32, ln = ol & 0xffffffff;
-    if (off < 0 || ln > 16 || off + ln > len) return false;
-    i128 v = (ln > 0 && (row[off] & 0x80)) ? -1 : 0;
-    for (int64_t k = 0; k < ln; k++) v = (v << 8) | row[off + k];
-    out->w = v; out->i = (int64_t)v;
-    return true;
-  }
-  switch (type) {
-    case SD_STRING: {
-      const int64_t ol = rd_i64(slot);
-      const int64_t off = ol >> 32, ln = ol & 0xffffffff;
-      if (off < 0 || off + ln > len) return false;
-      out->s.assign(reinterpret_cast<const char*>(row + off), (size_t)ln);
-      break;
-    }
-    case SD_BOOLEAN: out->i = slot[0] != 0; break;
-    case SD_BYTE: out->i = (int8_t)slot[0]; break;
-    case SD_SHORT: out->i = rd_i16(slot); break;
-    case SD_INT: case SD_DATE: out->i = rd_i32(slot); break;
-    case SD_FLOAT: out->d = rd_f32(slot); break;
-    case SD_DOUBLE: out->d = rd_f64(slot); break;
-    default: out->i = rd_i64(slot); break;
-  }
-  return true;
-}
-
-void emit_unsafe_row(std::vector<uint8_t>& out, const std::vector<int>& types, const std::vector<HVal>& vals) {
-  const int n = (int)types.size();
-  const int64_t bits = ((n + 63) / 64) * 8, fixed = bits + 8 * (int64_t)n;
-  int64_t var = 0;
-  for (int i = 0; i < n; i++) {
-    if (types[i] == SD_STRING && !vals[i].isnull) var += ((int64_t)vals[i].s.size() + 7) & ~int64_t(7);
-    if (ft_base(types[i]) == SD_DECIMAL && ft_precision(types[i]) > 18) var += 16;   // always reserved (UnsafeRowWriter.write(Decimal))
-  }
-  const int64_t sz = fixed + var;
-  const size_t base = out.size();
-  out.resize(base + 8 + sz, 0);
-  uint8_t* r = out.data() + base;
-  memcpy(r, &sz, 8);
-  r += 8;
-  int64_t voff = fixed;
-  for (int i = 0; i < n; i++) {
-    uint8_t* slot = r + bits + 8 * (int64_t)i;
-    if (ft_base(types[i]) == SD_DECIMAL) {
-      const bool wide = ft_precision(types[i]) > 18;
-      if (vals[i].isnull) {
-        r[i >> 3] |= (uint8_t)(1u << (i & 7));
-        if (wide) { const int64_t ol = voff << 32; memcpy(slot, &ol, 8); voff += 16; }   // offset kept, size 0
-        continue;
-      }
-      if (!wide) { const int64_t v = (int64_t)vals[i].w; memcpy(slot, &v, 8); continue; }
-      // BigInteger.toByteArray(): minimal big-endian two's complement
-      uint8_t be[16];
-      i128 v = vals[i].w;
-      for (int k = 15; k >= 0; k--) { be[k] = (uint8_t)(v & 0xff); v >>= 8; }
-      int first = 0;
-      while (first < 15 && ((be[first] == 0x00 && !(be[first + 1] & 0x80)) || (be[first] == 0xff && (be[first + 1] & 0x80)))) first++;
-      const int nb = 16 - first;
-      memcpy(r + voff, be + first, (size_t)nb);
-      const int64_t ol = (voff << 32) | (int64_t)nb;
-      memcpy(slot, &ol, 8);
-      voff += 16;
-      continue;
-    }
-    if (vals[i].isnull) { r[i >> 3] |= (uint8_t)(1u << (i & 7)); continue; }
-    switch (types[i]) {
-      case SD_STRING: {
-        const int64_t ol = (voff << 32) | (uint32_t)vals[i].s.size();
-        memcpy(slot, &ol, 8);
-        memcpy(r + voff, vals[i].s.data(), vals[i].s.size());
-        voff += ((int64_t)vals[i].s.size() + 7) & ~int64_t(7);
-        break;
-      }
-      case SD_BOOLEAN: slot[0] = vals[i].i != 0; break;
-      case SD_BYTE: { int8_t v = (int8_t)vals[i].i; memcpy(slot, &v, 1); break; }
-      case SD_SHORT: { int16_t v = (int16_t)vals[i].i; memcpy(slot, &v, 2); break; }
-      case SD_INT: case SD_DATE: { int32_t v = (int32_t)vals[i].i; memcpy(slot, &v, 4); break; }
-      case SD_FLOAT: { float v = (float)vals[i].d; memcpy(slot, &v, 4); break; }
-      case SD_DOUBLE: memcpy(slot, &vals[i].d, 8); break;
-      default: memcpy(slot, &vals[i].i, 8); break;
-    }
-  }
-}
 
 // ---- stats-row batch skipping (ColumnTableScan.generateStatPredicate, :820-963) -------------------
 struct Tri { bool isnull; bool v; };
@@ -637,9 +495,7 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
           // device record to point at, so the plan is refused rather than answering NULL for it
           bool order_input = false;
           for (const auto& m : sp.agg_map)
-            if (m.order_slot >= 0 && sp.slots[(size_t)m.order_slot].node >= 0 && sp.exprs[sp.slots[(size_t)m.order_slot].node].a == ts.col &&
-                m.buf_type == SD_STRING)
-              order_input = true;
+            if (m.family == AGG_ORDER && m.hold == HOLD_REF && sp.exprs[sp.slots[(size_t)m.value_slot].node].a == ts.col) order_input = true;
           if (order_input && ts.key < 0)
             for (int code = n + 1; code < (int)sc.dict_strings.size(); code++)
               if (code >= (int)sc.dict_rec_ptr.size() || sc.dict_rec_ptr[code] == 0)
@@ -1166,16 +1022,13 @@ int resolve_kernel(const sd_plan_desc& desc, const CodegenOptions& opt, int devi
   return 0;
 }
 
-// MIN / MAX over STRING: slots hold device addresses of [len][bytes] records -> their bytes, for every group at once
-typedef std::unordered_map<uint64_t, std::string> StrMap;
+// HOLD_REF values: slots hold device addresses of [len][bytes] records -> their bytes, for every group at once
 int fetch_agg_strings(sd_plan* p, const uint64_t* slots, size_t ngroups, StrMap& out) {
   const PlanSpec& sp = p->spec;
   const size_t ns = sp.slots.size();
   std::vector<int64_t> ptrs;
   for (auto& m : sp.agg_map) {
-    const int op = sp.slots[(size_t)m.value_slot].op;
-    const bool wide_order = m.order_slot >= 0 && m.buf_type == SD_DECIMAL && (m.buf_ps >> 8) > 18;   // FIRST / LAST: record address
-    if (m.buf_type != SD_STRING && op != SLOT_MIN_DEC && op != SLOT_MAX_DEC && !wide_order) continue;
+    if (m.hold != HOLD_REF) continue;
     for (size_t g = 0; g < ngroups; g++) { const uint64_t a = slots[g * ns + m.value_slot]; if (a && !out.count(a)) { out.emplace(a, std::string()); ptrs.push_back((int64_t)a); } }
   }
   if (ptrs.empty()) return 0;
@@ -1188,167 +1041,6 @@ int fetch_agg_strings(sd_plan* p, const uint64_t* slots, size_t ngroups, StrMap&
   if (rc) return rc;
   for (size_t i = 0; i < ptrs.size(); i++) out[(uint64_t)ptrs[i]] = strs[i];
   return 0;
-}
-
-// SUM / AVG buffers of a wide DECIMAL: a total of more than min(38, p + 10) digits is carried through partial rows (and every
-// merge of them) as pow10_128(precision), a value no in-range total reaches, so the final result is NULL however the rows
-// were split into partitions -- the rule one execution applies to all its rows
-static bool wide_sum_overflowed(i128 v, int prec) { return v >= pow10_128(prec) || v <= -pow10_128(prec); }
-// merges add partial totals exactly (each in-range one is below 2^127, so 64-bit halves summed in 128 bits cannot wrap);
-// the total is NULL when an input had overflowed or the exact sum of all of them needs more than `prec` digits
-static void wide_acc_add(HVal& b, const HVal& in, int prec) {
-  if (!b.acc) {
-    b.acc = true;
-    b.ovf = wide_sum_overflowed(b.w, prec);
-    b.acc_lo = (uint64_t)b.w;
-    b.acc_hi = b.w >> 64;
-  }
-  b.ovf = b.ovf || wide_sum_overflowed(in.w, prec);
-  b.acc_lo += (uint64_t)in.w;
-  b.acc_hi += in.w >> 64;
-}
-static void wide_acc_finish(HVal& b, int prec) {
-  if (!b.acc) return;
-  const i128 hi = b.acc_hi + (i128)(b.acc_lo >> 64);
-  const uint64_t lo = (uint64_t)b.acc_lo;
-  b.acc = false;
-  if (b.ovf || hi < -((i128)1 << 63) || hi >= ((i128)1 << 63)) b.w = pow10_128(prec);
-  else {
-    b.w = (i128)(((unsigned __int128)hi << 64) | lo);
-    if (wide_sum_overflowed(b.w, prec)) b.w = pow10_128(prec);
-  }
-  b.i = (int64_t)b.w;
-}
-
-// l3 * 2^96 + l2 * 2^64 + l1 * 2^32 + l0 (l0..l2: sums of unsigned 32-bit limbs, l3: sum of the signed top limbs); *fits = false
-// when the total is outside the int128 range
-static i128 limbs_to_i128(uint64_t l0, uint64_t l1, uint64_t l2, int64_t l3, bool* fits) {
-  uint64_t c = l0;
-  const uint64_t d0 = c & 0xffffffffull;
-  c = l1 + (c >> 32);
-  const uint64_t d1 = c & 0xffffffffull;
-  c = l2 + (c >> 32);
-  const uint64_t d2 = c & 0xffffffffull;
-  const i128 top = (i128)l3 + (i128)(c >> 32);
-  *fits = top >= -((i128)1 << 31) && top < ((i128)1 << 31);
-  if (!*fits) return 0;
-  const unsigned __int128 low = ((unsigned __int128)d2 << 64) | ((unsigned __int128)d1 << 32) | d0;
-  return (i128)(((unsigned __int128)top << 96) | low);
-}
-
-static double u2f_host(uint64_t u) { double d; memcpy(&d, &u, 8); return d; }
-
-// partial-row fields of one group from its slot values and its moment aggregates' K words `kw` (shared by the dense and the
-// hash paths)
-void append_agg_fields(const PlanSpec& sp, const uint64_t* sv, const uint64_t* kw, std::vector<HVal>& vals, const StrMap* strs = nullptr) {
-  for (auto& m : sp.agg_map) {
-    HVal v;
-    const uint64_t raw = sv[m.value_slot];
-    const int64_t cnt = m.count_slot >= 0 ? (int64_t)sv[m.count_slot] : 1;
-    if (m.order_slot >= 0) {   // FIRST / LAST: [value, valueSet] from the pair (order key, value)
-      const uint64_t key = sv[m.order_slot];
-      HVal set;
-      set.i = key != slot_initial(sp.slots[(size_t)m.order_slot].op);
-      if (!set.i || (key & 1ull)) v.isnull = true;   // no row, or the row's value is NULL
-      else if (m.buf_type == SD_STRING || (m.buf_type == SD_DECIMAL && (m.buf_ps >> 8) > 18)) {
-        const auto it = strs ? strs->find(raw) : StrMap::const_iterator();
-        if (!strs || it == strs->end()) v.isnull = true;
-        else if (m.buf_type == SD_STRING) v.s = it->second;
-        else if (it->second.empty() || it->second.size() > 16) v.isnull = true;
-        else { v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(it->second.data()), it->second.size()); v.i = (int64_t)v.w; }
-      } else if (type_is_fp(m.buf_type)) memcpy(&v.d, &raw, 8);
-      else { v.i = (int64_t)raw; v.w = v.i; }
-      vals.push_back(v);
-      vals.push_back(set);
-      continue;
-    }
-    if (m.buf_type == SD_STRING) {
-      if ((m.buf_nullable && cnt == 0) || raw == 0 || !strs) v.isnull = true;
-      else { auto it = strs->find(raw); if (it == strs->end()) v.isnull = true; else v.s = it->second; }
-      vals.push_back(v);
-      continue;
-    }
-    if (sp.slots[(size_t)m.value_slot].op == SLOT_MIN_DEC || sp.slots[(size_t)m.value_slot].op == SLOT_MAX_DEC) {   // wide MIN / MAX: record address
-      const auto it = strs ? strs->find(raw) : StrMap::const_iterator();
-      if ((m.buf_nullable && cnt == 0) || raw == 0 || !strs || it == strs->end() || it->second.empty() || it->second.size() > 16) v.isnull = true;
-      else { v.w = dec_from_bytes(reinterpret_cast<const uint8_t*>(it->second.data()), it->second.size()); v.i = (int64_t)v.w; }
-      vals.push_back(v);
-      continue;
-    }
-    if (m.limb_slot[0] >= 0) {   // SUM / AVG of a wide DECIMAL: four 32-bit limbs summed separately (sd_codegen.cpp build_slots)
-      bool fits = false;
-      v.w = limbs_to_i128(sv[m.limb_slot[0]], sv[m.limb_slot[1]], sv[m.limb_slot[2]], (int64_t)sv[m.limb_slot[3]], &fits);
-      if (!fits || wide_sum_overflowed(v.w, m.buf_ps >> 8)) v.w = pow10_128(m.buf_ps >> 8);   // overflowed: sticky (wide_sum_add)
-      v.i = (int64_t)v.w;
-      if (m.fn == SD_AGG_SUM) { if (m.buf_nullable && cnt == 0) v.isnull = true; vals.push_back(v); }
-      else { vals.push_back(v); HVal c; c.i = cnt; vals.push_back(c); }
-      continue;
-    }
-    if (is_moment(m.fn)) {   // Spark's buffers [n, avg, m2, (m3, (m4))] from n and S_j = sum (x - K)^j
-      const int order = moment_order(m.fn);
-      double b[5] = {0, 0, 0, 0, 0};
-      if (cnt > 0) {
-        const double n = (double)cnt, K = u2f_host(kw[m.shift]), S1 = u2f_host(sv[m.pow_slot[0]]), S2 = u2f_host(sv[m.pow_slot[1]]);
-        const double S3 = order >= 3 ? u2f_host(sv[m.pow_slot[2]]) : 0.0, S4 = order >= 4 ? u2f_host(sv[m.pow_slot[3]]) : 0.0;
-        const double d = S1 / n;
-        b[0] = n;
-        b[1] = K + d;
-        b[2] = S2 - n * d * d;
-        if (b[2] < 0) b[2] = 0;   // rounding; a NaN stays NaN
-        b[3] = S3 - 3 * d * S2 + 2 * n * d * d * d;
-        b[4] = S4 - 4 * d * S3 + 6 * d * d * S2 - 3 * n * d * d * d * d;
-      }
-      for (int j = 0; j <= order; j++) { HVal f; f.d = b[j]; vals.push_back(f); }
-      continue;
-    }
-    if (is_pair_agg(m.fn)) {   // Spark's buffers [n, xAvg, yAvg, ck, (xMk, yMk)] from n, S_x, S_y, S_xy (, S_xx, S_yy)
-      const bool corr = m.fn == SD_AGG_CORR;
-      double b[6] = {0, 0, 0, 0, 0, 0};
-      if (cnt > 0) {
-        const double n = (double)cnt, Kx = u2f_host(kw[m.shift]), Ky = u2f_host(kw[m.shift_y]);
-        const double Sx = u2f_host(sv[m.pair_slot[0]]), Sy = u2f_host(sv[m.pair_slot[1]]), Sxy = u2f_host(sv[m.pair_slot[2]]);
-        const double dx = Sx / n, dy = Sy / n;
-        b[0] = n;
-        if (!std::isfinite(Kx) || !std::isfinite(Ky) || !std::isfinite(Sx) || !std::isfinite(Sy)) {
-          // a counted row had a NaN or +-Inf x or y (its shifted value, or the group's K, is not finite): NaN, not the +-Inf
-          // some shifted sums would give
-          for (int j = 1; j < 6; j++) b[j] = NAN;
-        } else {
-          b[1] = Kx + dx;
-          b[2] = Ky + dy;
-          b[3] = Sxy - n * dx * dy;
-          if (corr) {
-            b[4] = std::max(0.0, u2f_host(sv[m.pair_slot[3]]) - n * dx * dx);   // >= 0 despite rounding (S_x, S_y are finite here)
-            b[5] = std::max(0.0, u2f_host(sv[m.pair_slot[4]]) - n * dy * dy);
-          }
-        }
-      }
-      for (int j = 0; j < (corr ? 6 : 4); j++) { HVal f; f.d = b[j]; vals.push_back(f); }
-      continue;
-    }
-    if (m.value_slot2 >= 0) {   // DECIMAL SUM / AVG: high and low halves summed separately (sd_codegen.cpp build_slots)
-      v.w = (i128)(int64_t)sv[m.value_slot] * ((i128)1 << 32) + (i128)(int64_t)sv[m.value_slot2];
-      v.i = (int64_t)v.w;
-      if (m.fn == SD_AGG_SUM) { if (m.buf_nullable && cnt == 0) v.isnull = true; vals.push_back(v); }
-      else { vals.push_back(v); HVal c; c.i = cnt; vals.push_back(c); }
-      continue;
-    }
-    switch (m.fn) {
-      case SD_AGG_COUNT_STAR: case SD_AGG_COUNT: v.i = (int64_t)raw; vals.push_back(v); break;
-      case SD_AGG_SUM:
-        if (m.buf_nullable && cnt == 0) v.isnull = true;
-        else if (m.buf_type == SD_DOUBLE) memcpy(&v.d, &raw, 8); else v.i = (int64_t)raw;
-        vals.push_back(v); break;
-      case SD_AGG_AVG: {
-        memcpy(&v.d, &raw, 8); vals.push_back(v);
-        HVal c; c.i = cnt; vals.push_back(c); break;
-      }
-      default:
-        if (m.buf_nullable && cnt == 0) v.isnull = true;
-        else if (type_is_fp(m.buf_type)) memcpy(&v.d, &raw, 8); else { v.i = (int64_t)raw; v.w = v.i; }
-        vals.push_back(v); break;
-    }
-  }
 }
 
 // compacted entries of a hash group table on the device: keys [count][nk], knull, vals [count][ns], K words [count][nsh]
@@ -2451,7 +2143,8 @@ int sd_rows_submit(sd_plan* p, const void* rows, int64_t len, int32_t nrows) {
   int64_t pos = 0;
   for (int i = 0; i < nrows; i++) {
     if (pos + 8 > len) return set_error(SD_ERR_INVALID, "sd_rows_submit: truncated row stream");
-    const int64_t sz = rd_i64(r + pos);
+    int64_t sz;
+    memcpy(&sz, r + pos, 8);
     if (sz < 0 || pos + 8 + sz > len) return set_error(SD_ERR_INVALID, "sd_rows_submit: bad row size");
     for (int c = 0; c < nc; c++)
       if (!unsafe_field(r + pos + 8, sz, nc, c, p->spec.cols[c].type, &colv[c][i])) return set_error(SD_ERR_INVALID, "sd_rows_submit: malformed UnsafeRow");
@@ -2514,17 +2207,14 @@ int sd_rows_submit(sd_plan* p, const void* rows, int64_t len, int32_t nrows) {
   return rc;
 }
 
-// ---- merge of partial rows (host; payload is a handful of rows) ------------------------------------------
-// evaluate = true : SnappyHashAggregateExec(Final) / CollectAggregateExec: merged buffers -> results (avg = sum / count)
-// evaluate = false: the merged PARTIAL rows (keys ++ buffers), what a combiner in front of the final stage emits
-static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t len, bool evaluate, std::vector<uint8_t>& out, int64_t* out_nrows);
-
+// ---- merge of partial rows (host, sd_aggregate.cpp) ------------------------------------------------------
 static int merge_to_caller(const PlanSpec& sp, const void* partial_rows, int64_t len, bool evaluate, void* out_rows, int64_t cap,
                            int64_t* out_len, int64_t* out_nrows) {
   if (!out_len) return set_error(SD_ERR_INVALID, "merge: null out_len");
   std::vector<uint8_t> out;
-  int rc = merge_rows_impl(sp, partial_rows, len, evaluate, out, out_nrows);
-  if (rc) return rc;
+  std::string err;
+  int rc = merge_rows(sp, partial_rows, len, evaluate, out, out_nrows, err);
+  if (rc) return set_error(rc, "%s", err.c_str());
   *out_len = (int64_t)out.size();
   if ((int64_t)out.size() > cap) return set_error(SD_ERR_OVERFLOW, "merge: output needs %zu bytes", out.size());
   if (!out.empty()) memcpy(out_rows, out.data(), out.size());
@@ -2560,220 +2250,6 @@ int sd_plan_partial_merge(sd_plan* p, const void* partial_rows, int64_t len, voi
                           int64_t* out_len, int64_t* out_nrows) {
   if (!p) return set_error(SD_ERR_INVALID, "null plan");
   return merge_to_caller(p->spec, partial_rows, len, false, out_rows, cap, out_len, out_nrows);
-}
-
-// CentralMomentAgg (Spark 2.1.1) on the buffers b[0..order] = [n, avg, m2, (m3, (m4))]: mergeExpressions ...
-static void moment_merge(HVal* b, const HVal* in, int order) {
-  const double n1 = b[0].d, n2 = in[0].d, n = n1 + n2;
-  const double delta = in[1].d - b[1].d, dN = n == 0.0 ? 0.0 : delta / n;
-  const double m2a = b[2].d, m2b = in[2].d;
-  const double m3a = order >= 3 ? b[3].d : 0.0, m3b = order >= 3 ? in[3].d : 0.0;
-  b[0].d = n;
-  b[1].d = b[1].d + dN * n2;
-  b[2].d = m2a + m2b + delta * dN * n1 * n2;
-  if (order >= 3) b[3].d = m3a + m3b + dN * dN * delta * n1 * n2 * (n1 - n2) + 3.0 * dN * (n1 * m2b - n2 * m2a);
-  if (order >= 4)
-    b[4].d = b[4].d + in[4].d + dN * dN * dN * delta * n1 * n2 * (n1 * n1 - n1 * n2 + n2 * n2) + 6.0 * dN * dN * (n1 * n1 * m2b + n2 * n2 * m2a) +
-             4.0 * dN * (n1 * m3b - n2 * m3a);
-}
-// Covariance / Corr (Spark 2.1.1) on the buffers [n, xAvg, yAvg, ck, (xMk, yMk)]: mergeExpressions ...
-static void pair_merge(HVal* b, const HVal* in, bool corr) {
-  const double n1 = b[0].d, n2 = in[0].d, n = n1 + n2;
-  const double dx = in[1].d - b[1].d, dxN = n == 0.0 ? 0.0 : dx / n;
-  const double dy = in[2].d - b[2].d, dyN = n == 0.0 ? 0.0 : dy / n;
-  b[0].d = n;
-  b[1].d = b[1].d + dxN * n2;
-  b[2].d = b[2].d + dyN * n2;
-  b[3].d = b[3].d + in[3].d + dx * dyN * n1 * n2;
-  if (corr) {
-    b[4].d = b[4].d + in[4].d + dx * dxN * n1 * n2;
-    b[5].d = b[5].d + in[5].d + dy * dyN * n1 * n2;
-  }
-}
-// ... and evaluateExpression: NULL without input
-static HVal pair_result(int fn, const HVal* b) {
-  HVal v;
-  const double n = b[0].d, ck = b[3].d;
-  if (n == 0.0) { v.isnull = true; return v; }
-  switch (fn) {
-    case SD_AGG_COVAR_POP: v.d = ck / n; break;
-    case SD_AGG_COVAR_SAMP: v.d = n == 1.0 ? NAN : ck / (n - 1.0); break;
-    default: v.d = n == 1.0 ? NAN : ck / std::sqrt(b[4].d * b[5].d); break;   // SD_AGG_CORR
-  }
-  return v;
-}
-// ... and evaluateExpression: NULL without input; stddev / variance are the SAMP forms
-static HVal moment_result(int fn, const HVal* b) {
-  HVal v;
-  const double n = b[0].d, m2 = b[2].d;
-  if (n == 0.0) { v.isnull = true; return v; }
-  switch (fn) {
-    case SD_AGG_VAR_POP: v.d = m2 / n; break;
-    case SD_AGG_STDDEV_POP: v.d = std::sqrt(m2 / n); break;
-    case SD_AGG_VAR_SAMP: v.d = n == 1.0 ? NAN : m2 / (n - 1.0); break;
-    case SD_AGG_STDDEV_SAMP: v.d = n == 1.0 ? NAN : std::sqrt(m2 / (n - 1.0)); break;
-    case SD_AGG_SKEWNESS: v.d = m2 == 0.0 ? NAN : std::sqrt(n) * b[3].d / std::sqrt(m2 * m2 * m2); break;
-    default: v.d = m2 == 0.0 ? NAN : n * b[4].d / (m2 * m2) - 3.0; break;   // SD_AGG_KURTOSIS
-  }
-  return v;
-}
-
-static int merge_rows_impl(const PlanSpec& sp, const void* partial_rows, int64_t len, bool evaluate, std::vector<uint8_t>& out, int64_t* out_nrows) {
-  out.clear();
-  if (sp.mode == MODE_PROJECT) {   // projected rows of several partitions: concatenation
-    const uint8_t* r = reinterpret_cast<const uint8_t*>(partial_rows);
-    int64_t pos = 0, n = 0;
-    while (pos + 8 <= len) {
-      const int64_t sz = rd_i64(r + pos);
-      if (sz < 0 || pos + 8 + sz > len) return set_error(SD_ERR_INVALID, "merge: bad row size");
-      pos += 8 + sz; n++;
-    }
-    out.assign(r, r + pos);
-    if (out_nrows) *out_nrows = n;
-    return 0;
-  }
-  const int nk = sp.out_keys();
-  const std::vector<int> types = partial_field_types(sp);
-  const int n = (int)types.size();
-  struct Group { std::vector<HVal> keys; std::vector<HVal> bufs; };
-  std::vector<Group> groups;   // insertion order
-  std::map<std::string, size_t> index;
-  const uint8_t* r = reinterpret_cast<const uint8_t*>(partial_rows);
-  int64_t pos = 0;
-  std::vector<HVal> f((size_t)n);
-  std::string key;
-  while (pos + 8 <= len) {
-    const int64_t sz = rd_i64(r + pos);
-    if (sz < 0 || pos + 8 + sz > len) return set_error(SD_ERR_INVALID, "sd_final_merge: bad row size");
-    for (int i = 0; i < n; i++) if (!unsafe_field(r + pos + 8, sz, n, i, types[i], &f[i])) return set_error(SD_ERR_INVALID, "sd_final_merge: malformed partial row");
-    key.clear();
-    for (int k = 0; k < nk; k++) {
-      key.push_back(f[k].isnull ? 'N' : 'V');
-      if (!f[k].isnull) {
-        if (types[k] == SD_STRING) { uint32_t l = (uint32_t)f[k].s.size(); key.append(reinterpret_cast<char*>(&l), 4); key.append(f[k].s); }
-        else if (type_is_fp(types[k])) { double d = f[k].d; if (d == 0.0) d = 0.0; if (std::isnan(d)) d = NAN; key.append(reinterpret_cast<char*>(&d), 8); }
-        else if (ft_base(types[k]) == SD_DECIMAL && ft_precision(types[k]) > 18) key.append(reinterpret_cast<const char*>(&f[k].w), 16);
-        else key.append(reinterpret_cast<const char*>(&f[k].i), 8);
-      }
-    }
-    auto it = nk > 0 ? index.find(key) : (groups.empty() ? index.end() : index.begin());
-    Group* g;
-    if (it == index.end()) {
-      index.emplace(key, groups.size());
-      groups.push_back(Group());
-      g = &groups.back();
-      g->keys.assign(f.begin(), f.begin() + nk);
-      g->bufs.assign(f.begin() + nk, f.end());
-    } else {
-      g = &groups[it->second];
-      int k = 0;
-      for (auto& m : sp.agg_map) {   // mergeExpressions of each function
-        HVal& b = g->bufs[k];
-        const HVal& in = f[nk + k];
-        if (is_moment(m.fn)) { moment_merge(&b, &in, moment_order(m.fn)); k += agg_buffer_fields(m.fn); continue; }
-        if (is_pair_agg(m.fn)) { pair_merge(&b, &in, m.fn == SD_AGG_CORR); k += agg_buffer_fields(m.fn); continue; }
-        if (is_order_agg(m.fn)) {   // First: valueSet.left ? left : right; Last: valueSet.right ? right : left; valueSet = left || right
-          HVal& bset = g->bufs[k + 1];
-          const HVal& inset = f[nk + k + 1];
-          if (is_last_agg(m.fn) ? inset.i != 0 : bset.i == 0) { b = in; bset.i = bset.i || inset.i; }
-          k += 2;
-          continue;
-        }
-        switch (m.fn) {
-          case SD_AGG_COUNT_STAR: case SD_AGG_COUNT: b.i += in.i; k++; break;
-          case SD_AGG_SUM:
-            if (!in.isnull) {
-              if (m.buf_type == SD_DOUBLE) b.d = (b.isnull ? 0.0 : b.d) + in.d;
-              else if (m.limb_slot[0] >= 0) { if (b.isnull) b.w = in.w; else wide_acc_add(b, in, m.buf_ps >> 8); }
-              else if (m.buf_type == SD_DECIMAL) { b.w = (b.isnull ? (i128)0 : b.w) + in.w; b.i = (int64_t)b.w; }
-              else b.i = (int64_t)((uint64_t)(b.isnull ? 0 : b.i) + (uint64_t)in.i);
-              b.isnull = false;
-            }
-            k++; break;
-          case SD_AGG_AVG:
-            if (m.limb_slot[0] >= 0) wide_acc_add(b, in, m.buf_ps >> 8);
-            else if (m.buf_type == SD_DECIMAL) { b.w += in.w; b.i = (int64_t)b.w; } else b.d += in.d;
-            g->bufs[k + 1].i += f[nk + k + 1].i; k += 2; break;
-          default:
-            if (!in.isnull) {
-              if (b.isnull) b = in;
-              else { const int c = cmp_hval(in, b, m.buf_type); if ((m.fn == SD_AGG_MIN && c < 0) || (m.fn == SD_AGG_MAX && c > 0)) b = in; }
-            }
-            k++; break;
-        }
-      }
-    }
-    pos += 8 + sz;
-  }
-  if (nk == 0 && groups.empty()) {   // no-key aggregate over no partitions: one row of empty buffers
-    Group g;
-    for (auto& m : sp.agg_map) {
-      HVal v;
-      if (m.fn == SD_AGG_SUM || m.fn == SD_AGG_MIN || m.fn == SD_AGG_MAX || is_order_agg(m.fn)) v.isnull = true;   // FIRST / LAST: [NULL, false]
-      g.bufs.push_back(v);
-      for (int j = 1; j < agg_buffer_fields(m.fn); j++) g.bufs.push_back(HVal());   // AVG's count, the moments' 0.0s
-    }
-    groups.push_back(g);
-  }
-  const std::vector<int> otypes = evaluate ? final_field_types(sp) : types;
-  std::vector<HVal> vals;
-  for (auto& g : groups) {
-    for (size_t a = 0, k = 0; a < sp.agg_map.size(); k += agg_buffer_fields(sp.agg_map[a].fn), a++)
-      if (sp.agg_map[a].limb_slot[0] >= 0) wide_acc_finish(g.bufs[k], sp.agg_map[a].buf_ps >> 8);
-    vals.assign(g.keys.begin(), g.keys.end());
-    if (!evaluate) vals.insert(vals.end(), g.bufs.begin(), g.bufs.end());
-    else {
-      int k = 0;
-      for (auto& m : sp.agg_map) {
-        if (is_moment(m.fn)) { vals.push_back(moment_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
-        if (is_pair_agg(m.fn)) { vals.push_back(pair_result(m.fn, &g.bufs[k])); k += agg_buffer_fields(m.fn); continue; }
-        if (is_order_agg(m.fn)) { vals.push_back(g.bufs[k]); k += 2; continue; }   // First / Last.evaluateExpression: value
-        if (m.fn == SD_AGG_AVG) {   // Average.evaluateExpression: sum / count, NULL when count == 0
-          HVal v;
-          const int64_t cnt = g.bufs[k + 1].i;
-          if (cnt == 0) v.isnull = true;
-          else if (m.limb_slot[0] >= 0) {
-            // the same quotient for a wide input, whose sum * 10^k may not fit 128 bits: q0 = sum / count, then the k more
-            // digits from the remainder (|remainder| * 10^k < 2^63 * 10^4); a q0 of more than precision - k digits cannot fit
-            const int ft = otypes[vals.size()], kk = ft_scale(ft) - (m.in_ps & 0xff), pr = ft_precision(ft);
-            const i128 sum = g.bufs[k].w, den = cnt, q0 = sum / den, r0 = sum % den;
-            // a sum of more than p + 10 digits is NULL: so is the average
-            if (wide_sum_overflowed(sum, m.buf_ps >> 8) || q0 >= pow10_128(pr - kk) || q0 <= -pow10_128(pr - kk)) v.isnull = true;
-            else {
-              const i128 num1 = r0 * pow10_128(kk);
-              i128 q = q0 * pow10_128(kk) + num1 / den, rem = num1 % den;
-              if (rem < 0) rem = -rem;
-              if (2 * rem >= den) q += (sum < 0 ? -1 : 1);
-              if (q >= pow10_128(pr) || q <= -pow10_128(pr)) v.isnull = true;
-              else { v.w = q; v.i = (int64_t)q; }
-            }
-          } else if (m.buf_type == SD_DECIMAL) {
-            // Cast(Cast(sum, DECIMAL(p+14,s+4)) / Cast(count, ...), DECIMAL(p+4,s+4)): the quotient at scale s+4, HALF_UP
-            const int ft = otypes[vals.size()];
-            const i128 num = g.bufs[k].w * pow10_128(ft_scale(ft) - (m.in_ps & 0xff)), den = cnt;
-            i128 q = num / den, rem = num % den;
-            if (rem < 0) rem = -rem;
-            if (2 * rem >= den) q += (num < 0 ? -1 : 1);
-            if (q >= pow10_128(ft_precision(ft)) || q <= -pow10_128(ft_precision(ft))) v.isnull = true;   // does not fit: NULL
-            else { v.w = q; v.i = (int64_t)q; }
-          } else v.d = g.bufs[k].d / (double)cnt;
-          vals.push_back(v);
-          k += 2;
-        } else {
-          HVal v = g.bufs[k];
-          if (m.fn == SD_AGG_SUM && m.buf_type == SD_DECIMAL && !v.isnull) {   // a sum that needs more than p+10 digits is NULL (changePrecision fails)
-            const i128 lim = pow10_128(m.buf_ps >> 8);
-            if (v.w >= lim || v.w <= -lim) v.isnull = true;
-          }
-          vals.push_back(v);
-          k++;
-        }
-      }
-    }
-    emit_unsafe_row(out, otypes, vals);
-  }
-  if (out_nrows) *out_nrows = (int64_t)groups.size();
-  return 0;
 }
 
 // ---- the one exchange of the path (SURVEY.md 8e): every partition's partial rows -> all ranks, merged ----------
@@ -2860,12 +2336,10 @@ static bool dense_exchange_eligible(const sd_plan* p) {
   if (sp.mode != MODE_NOKEY && sp.mode != MODE_GROUPS) return false;
   if (p->finished_nrows >= 0) return false;   // rows already materialised by an earlier call
   if (!sp.sets.empty()) return false;         // the ranks' rolled-up rows are gathered and merged by (keys, gid)
-  for (const auto& sl : sp.slots) if (sl.op == SLOT_MIN_STR || sl.op == SLOT_MAX_STR || sl.op == SLOT_MIN_DEC || sl.op == SLOT_MAX_DEC) return false;
-  for (const auto& m : sp.agg_map)   // FIRST / LAST values held as record addresses
-    if (m.order_slot >= 0 && (m.buf_type == SD_STRING || (m.buf_type == SD_DECIMAL && (m.buf_ps >> 8) > 18))) return false;
-  // limb sums are exact below 2^31 rows of ONE execution: summing them over the ranks could pass 2^64, so wide-DECIMAL sums
-  // take the by-value exchange, whose merge adds recombined 128-bit totals with an overflow check
-  for (const auto& sl : sp.slots) if (sl.gate >= GATE_LIMB0 && sl.gate <= GATE_LIMB3) return false;   // values live in this rank's HBM
+  // record addresses point into this rank's HBM; limb sums are exact below 2^31 rows of ONE execution, and summing them over
+  // the ranks could pass 2^64, so wide-DECIMAL sums take the by-value exchange, whose merge adds recombined 128-bit totals with
+  // an overflow check
+  for (const auto& m : sp.agg_map) if (m.hold == HOLD_REF || m.hold == HOLD_LIMBS) return false;
   return true;
 }
 
@@ -2993,8 +2467,9 @@ int sd_plan_exchange(sd_plan* p, sd_comm* c) {
   laps.lap(3, "decode-blobs");
   std::vector<uint8_t> merged;
   int64_t nrows = 0;
-  rc = merge_rows_impl(p->spec, all.data(), (int64_t)all.size(), false, merged, &nrows);
-  if (rc) return rc;
+  std::string err;
+  rc = merge_rows(p->spec, all.data(), (int64_t)all.size(), false, merged, &nrows, err);
+  if (rc) return set_error(rc, "%s", err.c_str());
   p->finished_rows.swap(merged);
   p->finished_nrows = nrows;
   p->dev_rows_len = -1;
