@@ -49,6 +49,7 @@ constexpr int MAX_RPT = 8;
 // bytes one row of a column occupies in a stage of the shared-memory ring (K_CODE: room for int32 indexes)
 constexpr int kind_stage_width(int k) { return (k == K_I64 || k == K_F64) ? 8 : (k == K_I32 || k == K_F32 || k == K_CODE) ? 4 : (k == K_I16) ? 2 : 1; }
 constexpr int MAX_STAGES = 12;
+constexpr int MAX_SCAN_COLS = 64;   // scan columns of one fused plan
 constexpr int RING_ALIGN_SLACK = 128;   // shared memory reserved to start the ring on a 128-byte boundary (sd_kernels.cuh)
 
 // bytes of TileSmem<PLAN> for a plan with nc scan columns (kept in sync with sd_kernels.cuh)
@@ -224,9 +225,17 @@ struct ScanArgs {
   int32_t shift_cache_off;        // MODE_GROUPS with moment aggregates, TABLE_PRIVATE / TABLE_SHARED_ATOMIC: byte offset in
                                   // dynamic shared memory of the CTA's copy of the K words, [ngroups][NSHIFT]; -1: none
   int32_t img_off;                // byte offset in dynamic shared memory of the per-chunk copies of the columns' img_tab
-                                  // (img_smem_words per column); -1: the staged loads read the verbatim values
+                                  // (img_smem_words per column, or RingArgs.img_col); -1: the staged loads read the verbatim values
   Literals lits;
 };
+// Ring layout of a launch of a dense group-by's two-CTA kernel (sd_kernels.cuh scan_aggregate_kernel_2cta), sized by the
+// widths the launch streams; every other kernel reads the verbatim layout as constants (stage_col_off / img_col_off)
+struct RingArgs {
+  int32_t stage_bytes;                    // bytes of one stage
+  int32_t stage_off[MAX_SCAN_COLS];       // byte offset of column c's region in a stage (128-byte aligned)
+  int32_t img_col[MAX_SCAN_COLS];         // word offset of column c's img_tab copy from ScanArgs.img_off
+};
+static_assert(sizeof(ScanArgs) + sizeof(RingArgs) <= 4096, "kernel parameters are limited to 4 KB");
 
 }  // namespace sd
 #endif

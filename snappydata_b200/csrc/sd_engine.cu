@@ -152,6 +152,10 @@ struct PathCounts {
   int32_t n[4] = {0, 0, 0, 0};
   // bytes of column values the launch reads: [0] every column verbatim, [1] scan images where the staged loads take them
   int64_t streamed[2] = {0, 0};
+  // per scan column, the widest element any staged batch of the launch streams: [0] with verbatim values, [1] with scan
+  // images where the batch has one; and the most img_tab words any batch's image of the column has
+  uint8_t width[2][MAX_SCAN_COLS] = {};
+  int32_t img_n[MAX_SCAN_COLS] = {};
 };
 
 // =====================================================================================================
@@ -172,6 +176,7 @@ struct sd_plan {
   int chunk_rows = CHUNK_ROWS;
   size_t last_smem = (size_t)-1;
   const KernelEntry* last_kernel = nullptr;
+  bool last_two_cta = false;      // last_kernel's two-CTA kernel was prepared
   int num_sms = 0;
   int smem_optin = 0;
   // literals
@@ -380,6 +385,9 @@ int remap_result(sd_plan* p, const int32_t* old_radix, int old_groups, const int
 }
 
 constexpr int REG_GROUPS_MAX = 8;
+// local memory the two-CTA kernel of a dense group-by may use beyond its one-CTA kernel: Q1's spills 8 bytes (three local
+// accesses in its SASS); plans whose per-row state does not fit 96 registers spill hundreds of bytes and stay at one CTA
+constexpr size_t TWO_CTA_SPILL_SLACK = 16;
 int resolve_kernel(const sd_plan_desc& desc, const CodegenOptions& opt, int device, KernelEntry* out, PlanSpec* spec_out);
 
 struct BuiltScan {
@@ -452,8 +460,15 @@ int build_scan(sd_plan* p, const std::vector<const StoredBatch*>& list, Arena& a
     for (int c = 0; c < nc; c++) {   // only the staged loads of the staged-only kernel variant read images (launch_scan)
       const int k = sp.kinds[c];
       const int64_t verbatim = k == K_CODE ? (dc[c].enc == ENC_DICTIONARY ? 2 : 4) : kind_stage_width(k);
+      const int64_t narrow = hdr->flags && dc[c].img ? dc[c].img_w : verbatim;
       out->paths.streamed[0] += verbatim * sb.num_rows;
-      out->paths.streamed[1] += (hdr->flags && dc[c].img ? dc[c].img_w : verbatim) * sb.num_rows;
+      out->paths.streamed[1] += narrow * sb.num_rows;
+      if (hdr->flags) {
+        PathCounts& pc = out->paths;
+        pc.width[0][c] = (uint8_t)std::max<int64_t>(pc.width[0][c], verbatim);
+        pc.width[1][c] = (uint8_t)std::max<int64_t>(pc.width[1][c], narrow);
+        if (dc[c].img) pc.img_n[c] = std::max(pc.img_n[c], dc[c].img_n);
+      }
     }
     // per-batch tables: [int32 offset x nt][pad 8][uint64 kpack x nt][tables]; every table is indexed by the
     // unified dictionary code; key maps of <= 8 codes are also packed one byte per code into kpack
@@ -752,7 +767,6 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   }
   int table_mode = TABLE_PRIVATE;
   int fresh = 0;
-  int target_ctas = std::max(1, sp.min_ctas);
   const int nshift = (int)sp.shifts.size();
   if (sp.mode == MODE_GROUPS && ngroups <= REG_GROUPS_MAX && k == &p->kernel && p->kernel.staged && getenv("SD_TUNE_REG_GROUPS") && nshift == 0) {
     // experimental (opt-in): measured slower than the private shared-memory tables, see DESIGN.md
@@ -762,51 +776,105 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
       sd_plan_desc dv = sp.desc_view();
       p->kernel_reg_state = resolve_kernel(dv, opt, p->device, &p->kernel_reg, nullptr) == 0 ? 1 : -1;
     }
+    // the accumulators are reduced through the ring, which keeps the verbatim layout below and at least two stages
     if (p->kernel_reg_state == 1 && 2 * p->kernel_reg.stage_bytes >= ne * THREADS * 8) {
       k = &p->kernel_reg;
       table_mode = TABLE_REGS;
-      target_ctas = 1;
     }
   }
+  // Two CTAs per SM for dense group-bys.  With images the per-row work, not the ring, bounds the kernel, and a second CTA
+  // doubles the consumer warps that hide its latency.  The staged-only variant has a kernel built for two CTAs
+  // (scan_aggregate_kernel_2cta, <= 96 registers) that reads the ring layout from the launch (RingArgs): each column's
+  // stage region sized by the widest element a batch of the launch streams (its scan image, or its verbatim width with
+  // dictionary codes at 2 or 4 bytes), each image table by the most entries a batch has.  A launch takes it when that
+  // kernel spills at most TWO_CTA_SPILL_SLACK bytes more than the one-CTA kernel, the tile state, the private table, the image tables and two compact
+  // stages fit half the SM, and the occupancy query agrees; otherwise it runs as before the two-CTA kernel existed: the
+  // plan's kernel, verbatim layout, one CTA.  SD_TUNE_RING_LAYOUT=verbatim or SD_TUNE_GROUP_CTAS=1 force the latter.
+  const char* layout_env = getenv("SD_TUNE_RING_LAYOUT");
+  const char* ctas_env = getenv("SD_TUNE_GROUP_CTAS");
+  const bool slow_variant = k == &p->variant[2] || k == &p->variant[3];
+  bool two_cta = sp.mode == MODE_GROUPS && table_mode != TABLE_REGS && (k->func2 || k->drv_func2) &&
+                 !(layout_env && !strcmp(layout_env, "verbatim")) && !(ctas_env && atoi(ctas_env) == 1);
+  if (two_cta) {
+    size_t local1 = 0, local2 = 0;
+    int rc = kernel_local_bytes(*k, false, &local1);
+    if (!rc) rc = kernel_local_bytes(*k, true, &local2);
+    if (rc) return rc;
+    two_cta = local2 <= local1 + TWO_CTA_SPILL_SLACK;
+  }
+  const bool want_img = k->staged && !slow_variant && paths.streamed[1] < paths.streamed[0];
+  const int nc = (int)sp.kinds.size();
+  RingArgs ring;
+  memset(&ring, 0, sizeof(ring));
   const size_t tile_smem = k->tile_smem;
   const size_t ring_fixed = 2 * MAX_STAGES * 8 + RING_ALIGN_SLACK;   // mbarriers + alignment of the ring
-  const size_t min_ring = k->staged ? ring_fixed + 2 * k->stage_bytes + 128 : 0;
-  size_t table_bytes = (size_t)std::max(ns, 1) * (THREADS / 32) * 8;
-  int shift_cache_off = -1;
-  if (sp.mode == MODE_GROUPS && table_mode != TABLE_REGS) {
-    // moment aggregates: the shared-memory tables come with the CTA's copy of the K words behind them
-    const size_t kc = (size_t)ngroups * nshift * 8;
-    const size_t priv = ne * THREADS * 8 + kc, shared = ne * 8 + kc;
-    // private copies are worth giving up CTAs per SM for; atomics are the last resort
-    while (target_ctas > 1 && tile_smem + priv + min_ring > (size_t)p->smem_optin / target_ctas - 1024) target_ctas--;
-    const size_t budget1 = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
-    if (tile_smem + priv + min_ring <= budget1) { table_mode = TABLE_PRIVATE; table_bytes = priv; }
-    else if (shared <= 64 * 1024 && tile_smem + shared + min_ring <= budget1) { table_mode = TABLE_SHARED_ATOMIC; table_bytes = shared; }
-    else { table_mode = TABLE_GLOBAL_ATOMIC; table_bytes = 64; }
-    if (nshift > 0 && table_mode != TABLE_GLOBAL_ATOMIC) shift_cache_off = (int)(tile_smem + table_bytes - kc);
-  }
-  const size_t budget = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
-  // the per-chunk copies of the image tables sit between the group table and the ring, when the batches have images, the
-  // kernel is the staged-only variant (the one with the per-row paths reads verbatim values) and the ring keeps at least
-  // two stages
-  int img_off = -1;
-  size_t img_end = tile_smem + table_bytes;
-  const bool slow_variant = k == &p->variant[2] || k == &p->variant[3];
-  if (k->staged && !slow_variant && paths.streamed[1] < paths.streamed[0]) {
+  size_t table_bytes, stage_bytes, ring_off, smem;
+  int target_ctas, shift_cache_off, img_off, nstages;
+  bool compact;
+  for (int attempt = two_cta ? 2 : 1;; attempt = 1) {
+    compact = attempt == 2;
+    // stage and image-table layout: compact (RingArgs) or verbatim (the kernel's constants)
+    stage_bytes = 0;
     size_t img_bytes = 0;
-    for (int kd : sp.kinds) img_bytes += 8 * (size_t)img_smem_words(kd);
-    const size_t off = (tile_smem + table_bytes + 15) & ~size_t(15);
-    if (((off + img_bytes + 127) & ~size_t(127)) + min_ring <= budget) { img_off = (int)off; img_end = off + img_bytes; }
-  }
-  size_t ring_off = (img_end + 127) & ~size_t(127);
-  int nstages = 0;
-  size_t smem = ring_off;
-  if (k->staged) {
-    if (ring_off + min_ring > (size_t)p->smem_optin) return set_error(SD_ERR_UNSUPPORTED, "plan does not fit the shared-memory ring (%zu bytes per stage)", k->stage_bytes);
-    const size_t avail = std::max(budget, ring_off + min_ring) - ring_off - ring_fixed;
-    nstages = (int)std::min<size_t>(MAX_STAGES, avail / k->stage_bytes);
-    if (const char* e = getenv("SD_TUNE_NSTAGES")) { int v = atoi(e); if (v >= 2 && v <= nstages) nstages = v; }
-    smem = ring_off + ring_fixed + (size_t)nstages * k->stage_bytes;
+    for (int c = 0; c < nc; c++) {
+      ring.stage_off[c] = (int32_t)stage_bytes;
+      ring.img_col[c] = (int32_t)(img_bytes / 8);
+      // + 128: a column with NULLs is copied from the 16-byte boundary below its first value of the tile, and every region
+      // stays 128-byte aligned for the bulk copies
+      stage_bytes += (size_t)k->tile_rows * (compact ? paths.width[want_img ? 1 : 0][c] : kind_stage_width(sp.kinds[c])) + 128;
+      img_bytes += 8 * (size_t)(compact ? paths.img_n[c] : img_smem_words(sp.kinds[c]));
+    }
+    ring.stage_bytes = (int32_t)stage_bytes;
+    target_ctas = table_mode == TABLE_REGS ? 1 : compact ? 2 : std::max(1, sp.min_ctas);
+    const size_t min_ring = k->staged ? ring_fixed + 2 * stage_bytes + 128 : 0;
+    table_bytes = (size_t)std::max(ns, 1) * (THREADS / 32) * 8;
+    shift_cache_off = -1;
+    auto img_fits = [&](size_t table, size_t budget) {   // the image tables sit between the group table and the ring
+      return ((((tile_smem + table + 15) & ~size_t(15)) + img_bytes + 127) & ~size_t(127)) + min_ring <= budget;
+    };
+    if (sp.mode == MODE_GROUPS && table_mode != TABLE_REGS) {
+      // moment aggregates: the shared-memory tables come with the CTA's copy of the K words behind them
+      const size_t kc = (size_t)ngroups * nshift * 8;
+      const size_t priv = ne * THREADS * 8 + kc, shared = ne * 8 + kc;
+      // private copies are worth giving up CTAs per SM for; atomics are the last resort
+      while (target_ctas > 1 && tile_smem + priv + min_ring > (size_t)p->smem_optin / target_ctas - 1024) target_ctas--;
+      const size_t budget1 = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
+      if (tile_smem + priv + min_ring <= budget1) { table_mode = TABLE_PRIVATE; table_bytes = priv; }
+      else if (shared <= 64 * 1024 && tile_smem + shared + min_ring <= budget1) { table_mode = TABLE_SHARED_ATOMIC; table_bytes = shared; }
+      else { table_mode = TABLE_GLOBAL_ATOMIC; table_bytes = 64; }
+      if (nshift > 0 && table_mode != TABLE_GLOBAL_ATOMIC) shift_cache_off = (int)(tile_smem + table_bytes - kc);
+    }
+    const size_t budget = (size_t)p->smem_optin / target_ctas - (target_ctas > 1 ? 1024 : 0);
+    if (compact && (target_ctas != 2 || table_mode != TABLE_PRIVATE || (want_img && !img_fits(table_bytes, budget)))) continue;
+    // the per-chunk copies of the image tables, when the batches have images, the kernel is the staged-only variant (the one
+    // with the per-row paths reads verbatim values) and the ring keeps at least two stages
+    img_off = -1;
+    size_t img_end = tile_smem + table_bytes;
+    if (want_img && img_fits(table_bytes, budget)) {
+      img_off = (int)((tile_smem + table_bytes + 15) & ~size_t(15));
+      img_end = img_off + img_bytes;
+    }
+    ring_off = (img_end + 127) & ~size_t(127);
+    nstages = 0;
+    smem = ring_off;
+    if (k->staged) {
+      if (ring_off + min_ring > (size_t)p->smem_optin) return set_error(SD_ERR_UNSUPPORTED, "plan does not fit the shared-memory ring (%zu bytes per stage)", stage_bytes);
+      const size_t avail = std::max(budget, ring_off + min_ring) - ring_off - ring_fixed;
+      nstages = (int)std::min<size_t>(MAX_STAGES, avail / stage_bytes);
+      if (const char* e = getenv("SD_TUNE_NSTAGES")) { int v = atoi(e); if (v >= 2 && v <= nstages) nstages = v; }
+      smem = ring_off + ring_fixed + (size_t)nstages * stage_bytes;
+    }
+    if (smem != p->last_smem || k != p->last_kernel || compact != p->last_two_cta) {
+      int occ = 0;
+      int rc = kernel_prepare(*k, compact, smem, &occ);
+      if (rc) return rc;
+      if (occ < 1) return set_error(SD_ERR_CUDA, "kernel does not fit on an SM (smem %zu)", smem);
+      p->max_ctas_per_sm = occ;
+      p->last_smem = smem;
+      p->last_kernel = k;
+      p->last_two_cta = compact;
+    }
+    if (!compact || p->max_ctas_per_sm >= 2) break;
   }
   if (p->active != k) { p->active = k; p->kernel_name = k->origin + ":" + k->name + (table_mode == TABLE_REGS ? "+regtable" : ""); }
   if (sp.mode == MODE_HASH) {
@@ -834,15 +902,6 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   p->ngroups = ngroups;
   memcpy(p->radix, radix, sizeof(radix));
 
-  if (smem != p->last_smem || k != p->last_kernel) {
-    int occ = 0;
-    int rc = kernel_prepare(*k, smem, &occ);
-    if (rc) return rc;
-    if (occ < 1) return set_error(SD_ERR_CUDA, "kernel does not fit on an SM (smem %zu)", smem);
-    p->max_ctas_per_sm = occ;
-    p->last_smem = smem;
-    p->last_kernel = k;
-  }
   const int occ = p->max_ctas_per_sm;
   const int grid = std::min(total_chunks, p->num_sms * occ);
   if (table_mode != TABLE_GLOBAL_ATOMIC && (size_t)grid * ne > p->partials_cap) {
@@ -909,7 +968,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
     args.lits.d[i] = p->lits[i].d;
     if (p->lits[i].is_null) args.lits.nullmask |= 1ull << i;
   }
-  void* kargs[] = {&args};
+  void* kargs[] = {&args, &ring};
   if (p->ev_used == p->ev_pairs.size() && p->ev_pairs.size() < 4096) {
     cudaEvent_t a = nullptr, b = nullptr;
     SD_CUDA(cudaEventCreate(&a));
@@ -919,7 +978,7 @@ int launch_scan(sd_plan* p, const void* d_batches, const int32_t* d_prefix, int 
   const bool own_pair = p->ev_used < p->ev_pairs.size();
   if (own_pair) SD_CUDA(cudaEventRecord(p->ev_pairs[p->ev_used].first, p->stream));
   if (!p->have_timing) SD_CUDA(cudaEventRecord(p->ev_start, p->stream));
-  { int rc = kernel_launch(*k, grid, smem, p->stream, kargs); if (rc) return rc; }
+  { int rc = kernel_launch(*k, compact, grid, smem, p->stream, kargs); if (rc) return rc; }
   if (p->launch_records.size() < (size_t)SDX_LAUNCH_LOG_MAX * SDX_LAUNCH_WORDS) {
     const int acc = sp.mode == MODE_NOKEY ? SDX_ACC_NOKEY : sp.mode == MODE_HASH ? SDX_ACC_HASH
                   : (sp.mode == MODE_PROJECT || sp.mode == MODE_MUTATE) ? SDX_ACC_ROWS

@@ -40,18 +40,23 @@ struct KernelEntry {
   int staged = 0;        // PLAN::STAGES > 0: producer warp + shared-memory ring (block = THREADS + 32)
   size_t stage_bytes = 0;
   int tile_rows = 0;     // THREADS * PLAN::RPT (set by the engine when it resolves the kernel)
+  // a dense group-by's staged-only variant: its kernel for two CTAs per SM (scan_aggregate_kernel_2cta), else null
+  const void* func2 = nullptr;
+  void* drv_func2 = nullptr;
   std::string origin;    // "aot" | "jit"
   std::string name;      // Plan_<fnv1a(signature)>: the generated struct's name
 };
 std::vector<KernelEntry>& kernel_registry();
 std::string plan_struct_name(const std::string& signature);
 struct AotRegistrar {
-  AotRegistrar(const char* signature, const void* func, size_t tile_smem, int staged, size_t stage_bytes);
+  AotRegistrar(const char* signature, const void* func, size_t tile_smem, int staged, size_t stage_bytes, const void* func2);
 };
 // set the dynamic shared-memory limit and query CTAs/SM; launch (runtime API for AOT, driver API for JIT)
-int kernel_prepare(const KernelEntry& k, size_t smem, int* ctas_per_sm);
+// two_cta: the entry's two-CTA kernel (func2 / drv_func2) instead of its kernel
+int kernel_prepare(const KernelEntry& k, bool two_cta, size_t smem, int* ctas_per_sm);
+int kernel_local_bytes(const KernelEntry& k, bool two_cta, size_t* bytes);   // local memory per thread (spills, stack)
 inline int kernel_block_threads(const KernelEntry& k) { return THREADS + (k.staged ? 32 : 0); }
-int kernel_launch(const KernelEntry& k, int grid, size_t smem, cudaStream_t stream, void** args);
+int kernel_launch(const KernelEntry& k, bool two_cta, int grid, size_t smem, cudaStream_t stream, void** args);
 // NVRTC path (sd_jit.cpp): compile `spec.source` against the embedded kernel headers.
 int jit_compile(const PlanSpec& spec, int device, KernelEntry& out);
 

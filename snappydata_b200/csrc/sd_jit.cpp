@@ -42,6 +42,7 @@ struct Dyn {
   CUresult (*ModuleLoadData)(CUmodule*, const void*) = nullptr;
   CUresult (*ModuleGetFunction)(CUfunction*, CUmodule, const char*) = nullptr;
   CUresult (*FuncSetAttribute)(CUfunction, CUfunction_attribute, int) = nullptr;
+  CUresult (*FuncGetAttribute)(int*, CUfunction_attribute, CUfunction) = nullptr;
   CUresult (*OccupancyMaxActiveBlocks)(int*, CUfunction, int, size_t) = nullptr;
   CUresult (*LaunchKernel)(CUfunction, unsigned, unsigned, unsigned, unsigned, unsigned, unsigned, unsigned, CUstream, void**, void**) = nullptr;
   CUresult (*GetErrorStringDrv)(CUresult, const char**) = nullptr;
@@ -63,7 +64,7 @@ Dyn& dyn() {
     NV(AddNameExpression) NV(GetLoweredName) NV(GetErrorString)
 #undef NV
 #define CUF(field, sym) *(void**)(&d.field) = dlsym(d.cuda, sym); if (!d.field) { d.why = sym " missing"; return; }
-    CUF(ModuleLoadData, "cuModuleLoadData") CUF(ModuleGetFunction, "cuModuleGetFunction") CUF(FuncSetAttribute, "cuFuncSetAttribute")
+    CUF(ModuleLoadData, "cuModuleLoadData") CUF(ModuleGetFunction, "cuModuleGetFunction") CUF(FuncSetAttribute, "cuFuncSetAttribute") CUF(FuncGetAttribute, "cuFuncGetAttribute")
     CUF(OccupancyMaxActiveBlocks, "cuOccupancyMaxActiveBlocksPerMultiprocessor") CUF(LaunchKernel, "cuLaunchKernel")
     CUF(GetErrorStringDrv, "cuGetErrorString")
 #undef CUF
@@ -80,32 +81,54 @@ const char* drv_err(CUresult r) {
 
 }  // namespace
 
-int kernel_prepare(const KernelEntry& k, size_t smem, int* ctas_per_sm) {
-  if (k.func) {
-    SD_CUDA(cudaFuncSetAttribute(k.func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+int kernel_prepare(const KernelEntry& k, bool two_cta, size_t smem, int* ctas_per_sm) {
+  const void* func = two_cta ? k.func2 : k.func;
+  void* drv_func = two_cta ? k.drv_func2 : k.drv_func;
+  if (func) {
+    SD_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // ask for the largest shared-memory carveout so that several CTAs with private group tables fit per SM
-    SD_CUDA(cudaFuncSetAttribute(k.func, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    SD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k.func, kernel_block_threads(k), smem));
+    SD_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    SD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, func, kernel_block_threads(k), smem));
     return 0;
   }
   Dyn& d = dyn();
-  if (!d.ok || !k.drv_func) return set_error(SD_ERR_CUDA, "no kernel for this plan: %s", d.why.c_str());
-  CUresult r = d.FuncSetAttribute((CUfunction)k.drv_func, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+  if (!d.ok || !drv_func) return set_error(SD_ERR_CUDA, "no kernel for this plan: %s", d.why.c_str());
+  CUresult r = d.FuncSetAttribute((CUfunction)drv_func, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
   if (r != CUDA_SUCCESS) return set_error(SD_ERR_CUDA, "cuFuncSetAttribute: %s", drv_err(r));
-  d.FuncSetAttribute((CUfunction)k.drv_func, CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, 100);
-  r = d.OccupancyMaxActiveBlocks(ctas_per_sm, (CUfunction)k.drv_func, kernel_block_threads(k), smem);
+  d.FuncSetAttribute((CUfunction)drv_func, CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, 100);
+  r = d.OccupancyMaxActiveBlocks(ctas_per_sm, (CUfunction)drv_func, kernel_block_threads(k), smem);
   if (r != CUDA_SUCCESS) return set_error(SD_ERR_CUDA, "cuOccupancyMaxActiveBlocksPerMultiprocessor: %s", drv_err(r));
   return 0;
 }
 
-int kernel_launch(const KernelEntry& k, int grid, size_t smem, cudaStream_t stream, void** args) {
-  if (k.func) {
-    SD_CUDA(cudaLaunchKernel(k.func, dim3(grid), dim3(kernel_block_threads(k)), args, smem, stream));
+int kernel_local_bytes(const KernelEntry& k, bool two_cta, size_t* bytes) {
+  const void* func = two_cta ? k.func2 : k.func;
+  void* drv_func = two_cta ? k.drv_func2 : k.drv_func;
+  if (func) {
+    cudaFuncAttributes a;
+    SD_CUDA(cudaFuncGetAttributes(&a, func));
+    *bytes = a.localSizeBytes;
     return 0;
   }
   Dyn& d = dyn();
-  if (!d.ok || !k.drv_func) return set_error(SD_ERR_CUDA, "no kernel for this plan: %s", d.why.c_str());
-  CUresult r = d.LaunchKernel((CUfunction)k.drv_func, grid, 1, 1, kernel_block_threads(k), 1, 1, (unsigned)smem, (CUstream)stream, args, nullptr);
+  if (!d.ok || !drv_func) return set_error(SD_ERR_CUDA, "no kernel for this plan: %s", d.why.c_str());
+  int v = 0;
+  CUresult r = d.FuncGetAttribute(&v, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, (CUfunction)drv_func);
+  if (r != CUDA_SUCCESS) return set_error(SD_ERR_CUDA, "cuFuncGetAttribute: %s", drv_err(r));
+  *bytes = (size_t)v;
+  return 0;
+}
+
+int kernel_launch(const KernelEntry& k, bool two_cta, int grid, size_t smem, cudaStream_t stream, void** args) {
+  const void* func = two_cta ? k.func2 : k.func;
+  void* drv_func = two_cta ? k.drv_func2 : k.drv_func;
+  if (func) {
+    SD_CUDA(cudaLaunchKernel(func, dim3(grid), dim3(kernel_block_threads(k)), args, smem, stream));
+    return 0;
+  }
+  Dyn& d = dyn();
+  if (!d.ok || !drv_func) return set_error(SD_ERR_CUDA, "no kernel for this plan: %s", d.why.c_str());
+  CUresult r = d.LaunchKernel((CUfunction)drv_func, grid, 1, 1, kernel_block_threads(k), 1, 1, (unsigned)smem, (CUstream)stream, args, nullptr);
   if (r != CUDA_SUCCESS) return set_error(SD_ERR_CUDA, "cuLaunchKernel: %s", drv_err(r));
   return 0;
 }
@@ -123,6 +146,10 @@ int jit_compile(const PlanSpec& spec, int device, KernelEntry& out) {
   nvrtcResult nr = d.CreateProgram(&prog, src.c_str(), (spec.struct_name + ".cu").c_str(), 2, headers, names);
   if (nr != NVRTC_SUCCESS) return set_error(SD_ERR_CUDA, "nvrtcCreateProgram: %s", d.GetErrorString(nr));
   d.AddNameExpression(prog, name_expr.c_str());
+  // a dense group-by's staged-only variant has a second kernel for two CTAs per SM (sd_kernels.cuh TwoCtaKernel)
+  const bool two_cta = spec.mode == MODE_GROUPS && !spec.slow_paths && spec.stages > 0 && spec.reg_groups == 0;
+  const std::string name_expr2 = "sd::scan_aggregate_kernel_2cta<" + spec.struct_name + ">";
+  if (two_cta) d.AddNameExpression(prog, name_expr2.c_str());
   // -lineinfo adds ~50 % to the compile: only when a profile of a JIT kernel is wanted (SD_JIT_LINEINFO=1)
   // -device-int128: 128-bit integers of the wide-DECIMAL helpers in sd_kernels.cuh (nvcc allows them on sm_90a by default)
   std::vector<std::string> optv = {"--gpu-architecture=sm_90a", "-std=c++17", "--fmad=false", "-default-device", "-device-int128"};
@@ -156,13 +183,21 @@ int jit_compile(const PlanSpec& spec, int device, KernelEntry& out) {
   CUmodule mod;
   CUresult r = d.ModuleLoadData(&mod, cubin.data());
   if (r != CUDA_SUCCESS) { d.DestroyProgram(&prog); return set_error(SD_ERR_CUDA, "cuModuleLoadData: %s", drv_err(r)); }
-  CUfunction fn;
+  CUfunction fn, fn2 = nullptr;
   r = d.ModuleGetFunction(&fn, mod, lowered);
+  if (r == CUDA_SUCCESS && two_cta) {
+    const char* lowered2 = nullptr;
+    nr = d.GetLoweredName(prog, name_expr2.c_str(), &lowered2);
+    if (nr != NVRTC_SUCCESS || !lowered2) { d.DestroyProgram(&prog); return set_error(SD_ERR_CUDA, "nvrtcGetLoweredName failed"); }
+    r = d.ModuleGetFunction(&fn2, mod, lowered2);
+  }
   d.DestroyProgram(&prog);
   if (r != CUDA_SUCCESS) return set_error(SD_ERR_CUDA, "cuModuleGetFunction: %s", drv_err(r));
   out.signature = spec.signature;
   out.func = nullptr;
   out.drv_func = (void*)fn;
+  out.func2 = nullptr;
+  out.drv_func2 = (void*)fn2;
   out.tile_smem = ((size_t)tile_smem_bytes((int)spec.cols.size(), spec.rpt) + 15) & ~size_t(15);
   out.origin = "jit";
   out.name = spec.struct_name;

@@ -834,6 +834,28 @@ __device__ __forceinline__ void verify_all(const AllCols<PLAN, Seq<Cs...>>& a, c
   }
   (void)dummy;
 }
+#ifndef SD_EXP_SKIP_ROWS
+#define SD_EXP_SKIP_ROWS 0
+#endif
+#ifndef SD_EXP_SINK_GROUPS
+#define SD_EXP_SINK_GROUPS 0
+#endif
+// SD_EXP_SKIP_ROWS (diagnostic builds only): a tile's loads end in a register sink instead of the row loop
+template <class PLAN, int C>
+__device__ __forceinline__ void fold_col(const ColRegs<PLAN, C>& a, uint64_t& sink) {
+  sink ^= a.nullmask;
+#pragma unroll
+  for (int r = 0; r < PLAN::RPT; r++) {
+    unsigned long long x = 0;
+    memcpy(&x, &a.v[r], sizeof(a.v[r]));
+    sink ^= x;
+  }
+}
+template <class PLAN, int... Cs>
+__device__ __forceinline__ void fold_all(const AllCols<PLAN, Seq<Cs...>>& a, uint64_t& sink, Seq<Cs...>) {
+  int dummy[] = {0, (fold_col<PLAN, Cs>(static_cast<const ColRegs<PLAN, Cs>&>(a), sink), 0)...};
+  (void)dummy;
+}
 template <class PLAN, int... Cs>
 __device__ __forceinline__ void clear_upd_bits(const DevBatch<PLAN::NC>& b, TileSmem<PLAN>& sm, Seq<Cs...>) {
   const int tid = threadIdx.x;
@@ -891,7 +913,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 // consumer-only CTA barrier (the producer warp never joins it)
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(THREADS) : "memory"); }
 
-// byte offset of column C's tile inside a stage (sized by the verbatim width: a scan image is never wider)
+// byte offset of column C's tile inside a stage of the verbatim layout (every column at its kind's widest element)
 template <class PLAN>
 __host__ __device__ constexpr int stage_col_off(int c) {
   int off = 0;
@@ -900,7 +922,7 @@ __host__ __device__ constexpr int stage_col_off(int c) {
   for (int i = 0; i < c; i++) off += THREADS * PLAN::RPT * kind_stage_width(PLAN::kind(i)) + 128;
   return off;
 }
-// word offset of column C's img_tab copy in the kernel's shared-memory image tables (ScanArgs.img_off)
+// word offset of column C's img_tab copy in the kernel's shared-memory image tables (ScanArgs.img_off) in the verbatim layout
 template <class PLAN>
 __host__ __device__ constexpr int img_col_off(int c) {
   int off = 0;
@@ -911,6 +933,14 @@ template <class PLAN>
 struct StageInfo {
   static constexpr int BYTES = stage_col_off<PLAN>(PLAN::NC);
 };
+// The ring layout a kernel reads (RT): the launch's (RingArgs, sized by what the launch streams: the two-CTA kernel of a
+// dense group-by), or the verbatim layout as constants (every other kernel)
+template <class PLAN, bool RT, int C>
+__device__ __forceinline__ int stage_off(const RingArgs& r) { return RT ? r.stage_off[C] : stage_col_off<PLAN>(C); }
+template <class PLAN, bool RT>
+__device__ __forceinline__ int stage_size(const RingArgs& r) { return RT ? r.stage_bytes : StageInfo<PLAN>::BYTES; }
+template <class PLAN, bool RT, int C>
+__device__ __forceinline__ int img_col(const RingArgs& r) { return RT ? r.img_col[C] : img_col_off<PLAN>(C); }
 
 // one bit per scan column: 32 bits for plans of <= 32 columns (the common case keeps its register budget), 64 beyond
 template <bool WIDE> struct CMaskT { typedef uint32_t T; };
@@ -966,15 +996,15 @@ __device__ __forceinline__ void col_copy_range(const int32_t* tile_nulls, const 
   *src_off = off & ~int64_t(15);
   *bytes = cnt > 0 ? (uint32_t)(((off & 15) + (int64_t)cnt * w + 15) & ~int64_t(15)) : 0u;   // buffers are padded: over-reading is safe
 }
-template <class PLAN, int... Cs>
-__device__ __forceinline__ void issue_tile_copies(const ProducerCols<PLAN::NC>& pc, const ColModes<PLAN>& cm, int64_t tile_start, int rows, uint8_t* stage, uint64_t* bar, Seq<Cs...>) {
+template <class PLAN, bool RT, int... Cs>
+__device__ __forceinline__ void issue_tile_copies(const RingArgs& a, const ProducerCols<PLAN::NC>& pc, const ColModes<PLAN>& cm, int64_t tile_start, int rows, uint8_t* stage, uint64_t* bar, Seq<Cs...>) {
   int64_t off[PLAN::NC > 0 ? PLAN::NC : 1];
   uint32_t bytes[PLAN::NC > 0 ? PLAN::NC : 1];
   uint32_t total = 0;
   int d0[] = {0, (col_copy_range<PLAN, Cs>(pc.tile_nulls[Cs], cm, tile_start, rows, &off[Cs], &bytes[Cs]), total += bytes[Cs], 0)...};
   (void)d0;
   mbar_expect_tx(bar, total);
-  int d1[] = {0, ((!PLAN::col_nullable(Cs) || bytes[Cs]) ? (bulk_g2s(stage + stage_col_off<PLAN>(Cs), pc.data[Cs] + off[Cs], bytes[Cs], bar), 0) : 0)...};
+  int d1[] = {0, ((!PLAN::col_nullable(Cs) || bytes[Cs]) ? (bulk_g2s(stage + stage_off<PLAN, RT, Cs>(a), pc.data[Cs] + off[Cs], bytes[Cs], bar), 0) : 0)...};
   (void)d1;
 }
 
@@ -986,14 +1016,14 @@ __device__ __forceinline__ T img_value(const uint64_t* tab, uint32_t x) {
   return (T)((int64_t)tab[0] + (int64_t)x);   // wraps to the element width exactly as the image builder verified
 }
 // consumer: registers <- stage (conflict-free: consecutive lanes read consecutive 16/8/4/2 bytes)
-template <class PLAN, int C>
-__device__ __forceinline__ void load_col_staged(const ColModes<PLAN>& cm, const uint64_t* imgsm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
+template <class PLAN, bool RT, int C>
+__device__ __forceinline__ void load_col_staged(const RingArgs& a, const ColModes<PLAN>& cm, const uint64_t* imgsm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
   typedef typename KindT<PLAN::kind(C)>::T T;
   constexpr int K = PLAN::kind(C);
-  const uint8_t* base = stage + stage_col_off<PLAN>(C);
+  const uint8_t* base = stage + stage_off<PLAN, RT, C>(a);
   regs.nullmask = 0;
   if (kind_has_image(K) && ((cm.img >> C) & 1)) {
-    const uint64_t* tab = imgsm + img_col_off<PLAN>(C);
+    const uint64_t* tab = imgsm + img_col<PLAN, RT, C>(a);
     const bool w1 = (cm.w1 >> C) & 1;
 #pragma unroll
     for (int u = 0; u < PLAN::RPT / 2; u++) {
@@ -1040,15 +1070,15 @@ __device__ __forceinline__ void load_col_staged(const ColModes<PLAN>& cm, const 
 }
 // consumer, column with NULLs: row -> (is null, value index) through the null words; the value sits in the stage at
 // [shift + (k - first) * w] where `first` is the tile's first stored value
-template <class PLAN, int C>
-__device__ __forceinline__ void load_col_staged_nulls(const DevCol& col, const ColModes<PLAN>& cm, int64_t tile_start, int num_rows,
+template <class PLAN, bool RT, int C>
+__device__ __forceinline__ void load_col_staged_nulls(const RingArgs& a, const DevCol& col, const ColModes<PLAN>& cm, int64_t tile_start, int num_rows,
                                                       const TileSmem<PLAN>& sm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
   typedef typename KindT<PLAN::kind(C)>::T T;
   constexpr int K = PLAN::kind(C);
   const int w = col_width<PLAN, C>(cm);   // (a column with NULLs in the batch has no image)
   const int n0 = col.tile_nulls[tile_start / NULL_PREFIX_ROWS];
   const int64_t first = tile_start - n0;
-  const uint8_t* base = stage + stage_col_off<PLAN>(C) + ((first * w) & 15);
+  const uint8_t* base = stage + stage_off<PLAN, RT, C>(a) + ((first * w) & 15);
   regs.nullmask = 0;
   // nulls before each 64-row word of the tile, computed BY EVERY WARP FOR ITSELF with shuffles (no shared memory, no CTA
   // barrier: warp-0-only preparation with two barriers per tile kept this path at a quarter of the roofline).  The rows of
@@ -1086,21 +1116,21 @@ __device__ __forceinline__ void load_col_staged_nulls(const DevCol& col, const C
     regs.nullmask |= (isnull ? 1u : 0u) << r;
   }
 }
-template <class PLAN, int C>
-__device__ __forceinline__ void load_col_staged_any(const DevCol& col, const ColModes<PLAN>& cm, const uint64_t* imgsm, int64_t tile_start, int num_rows,
+template <class PLAN, bool RT, int C>
+__device__ __forceinline__ void load_col_staged_any(const RingArgs& a, const DevCol& col, const ColModes<PLAN>& cm, const uint64_t* imgsm, int64_t tile_start, int num_rows,
                                                     const TileSmem<PLAN>& sm, const uint8_t* stage, ColRegs<PLAN, C>& regs) {
-  if (PLAN::col_nullable(C) && col.nulls) load_col_staged_nulls<PLAN, C>(col, cm, tile_start, num_rows, sm, stage, regs);
-  else load_col_staged<PLAN, C>(cm, imgsm, stage, regs);
+  if (PLAN::col_nullable(C) && col.nulls) load_col_staged_nulls<PLAN, RT, C>(a, col, cm, tile_start, num_rows, sm, stage, regs);
+  else load_col_staged<PLAN, RT, C>(a, cm, imgsm, stage, regs);
 }
-template <class PLAN, int... Cs>
-__device__ __forceinline__ void load_all_staged_nulls(const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, const uint64_t* imgsm, int64_t tile_start, const TileSmem<PLAN>& sm,
+template <class PLAN, bool RT, int... Cs>
+__device__ __forceinline__ void load_all_staged_nulls(const RingArgs& a, const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, const uint64_t* imgsm, int64_t tile_start, const TileSmem<PLAN>& sm,
                                                       const uint8_t* stage, AllCols<PLAN, Seq<Cs...>>& regs, Seq<Cs...>) {
-  int dummy[] = {0, (load_col_staged_any<PLAN, Cs>(b.cols[Cs], cm, imgsm, tile_start, b.num_rows, sm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
+  int dummy[] = {0, (load_col_staged_any<PLAN, RT, Cs>(a, b.cols[Cs], cm, imgsm, tile_start, b.num_rows, sm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
   (void)dummy;
 }
-template <class PLAN, int... Cs>
-__device__ __forceinline__ void load_all_staged(const ColModes<PLAN>& cm, const uint64_t* imgsm, const uint8_t* stage, AllCols<PLAN, Seq<Cs...>>& regs, Seq<Cs...>) {
-  int dummy[] = {0, (load_col_staged<PLAN, Cs>(cm, imgsm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
+template <class PLAN, bool RT, int... Cs>
+__device__ __forceinline__ void load_all_staged(const RingArgs& a, const ColModes<PLAN>& cm, const uint64_t* imgsm, const uint8_t* stage, AllCols<PLAN, Seq<Cs...>>& regs, Seq<Cs...>) {
+  int dummy[] = {0, (load_col_staged<PLAN, RT, Cs>(a, cm, imgsm, stage, static_cast<ColRegs<PLAN, Cs>&>(regs)), 0)...};
   (void)dummy;
 }
 
@@ -1181,18 +1211,19 @@ __device__ __forceinline__ ColModes<PLAN> col_modes(const DevBatch<PLAN::NC>& b,
   return cm;
 }
 // the chunk's img_tab words -> shared memory (the caller brackets this with consumer barriers)
-template <class PLAN, int... Cs>
-__device__ __forceinline__ void load_img_tables(const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, uint64_t* imgsm, Seq<Cs...>) {
+template <class PLAN, bool RT, int... Cs>
+__device__ __forceinline__ void load_img_tables(const RingArgs& a, const DevBatch<PLAN::NC>& b, const ColModes<PLAN>& cm, uint64_t* imgsm, Seq<Cs...>) {
   int dummy[] = {0, (kind_has_image(PLAN::kind(Cs)) && ((cm.img >> Cs) & 1)
-                     ? ([&] { for (int i = threadIdx.x; i < b.cols[Cs].img_n; i += THREADS) imgsm[img_col_off<PLAN>(Cs) + i] = __ldg(&b.cols[Cs].img_tab[i]); }(), 0) : 0)...};
+                     ? ([&] { for (int i = threadIdx.x; i < b.cols[Cs].img_n; i += THREADS) imgsm[img_col<PLAN, RT, Cs>(a) + i] = __ldg(&b.cols[Cs].img_tab[i]); }(), 0) : 0)...};
   (void)dummy;
 }
 
 // ================================================================================================
 // The kernel.  dynamic shared memory: [TileSmem<PLAN>] [private group tables | reduction scratch]
 // ================================================================================================
-template <class PLAN>
-__global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::MIN_CTAS) scan_aggregate_kernel(const ScanArgs args) {
+// (the body of both kernels below; RT: the ring layout of the launch, `rl`, instead of the verbatim one)
+template <class PLAN, bool RT>
+__device__ __forceinline__ void scan_aggregate(const ScanArgs args, const RingArgs rl) {
   typedef typename MakeSeq<PLAN::NC>::type ColSeq;
   constexpr int NSLOT = PLAN::NSLOT;
   constexpr int RPT = PLAN::RPT;
@@ -1242,7 +1273,7 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
             const int64_t tile_start = (int64_t)tile * TILE_ROWS;
             const int rows = min(TILE_ROWS, num_rows - (int)tile_start);
             mbar_wait(&empty_bar[stage], phase ^ 1u);
-            issue_tile_copies<PLAN>(pc, cm, tile_start, rows, ring + (size_t)stage * StageInfo<PLAN>::BYTES, &full_bar[stage], ColSeq());
+            issue_tile_copies<PLAN, RT>(rl, pc, cm, tile_start, rows, ring + (size_t)stage * stage_size<PLAN, RT>(rl), &full_bar[stage], ColSeq());
             if (++stage == nstages) { stage = 0; phase ^= 1u; }
           }
         }
@@ -1298,6 +1329,12 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     }
   }
   unsigned long long n_scanned = 0, n_passed = 0;   // flushed from 32-bit per-chunk counters
+#if SD_EXP_SKIP_ROWS || SD_EXP_SINK_GROUPS
+  uint64_t exp_sink = 0;
+  uint64_t exp_acc[NSLOT > 0 ? NSLOT : 1];
+#pragma unroll
+  for (int s = 0; s < NSLOT; s++) exp_acc[s] = 0;
+#endif
 
   RowCtx ctx;
   ctx.L = &args.lits;
@@ -1322,7 +1359,7 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
     const ColModes<PLAN> cm = col_modes<PLAN>(b, args.img_off >= 0, ColSeq());
     if (PLAN::STAGES > 0 && !PLAN::SLOW_PATHS && fast && cm.img && lo != img_batch) {
       consumer_sync();   // every consumer is done with the previous batch's tables
-      load_img_tables<PLAN>(b, cm, reinterpret_cast<uint64_t*>(smem_raw + args.img_off), ColSeq());
+      load_img_tables<PLAN, RT>(rl, b, cm, reinterpret_cast<uint64_t*>(smem_raw + args.img_off), ColSeq());
       consumer_sync();
       img_batch = lo;
     }
@@ -1342,8 +1379,8 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
         if (PLAN::STAGES > 0) {
           mbar_wait(&full_bar[c_stage], c_phase);   // (the NULL-aware loads derive their word prefixes per warp: no barrier here)
           const uint64_t* imgsm = reinterpret_cast<const uint64_t*>(smem_raw + args.img_off);   // (read only where cm.img)
-          if (with_nulls) load_all_staged_nulls<PLAN>(b, cm, imgsm, tile_start, sm, ring + (size_t)c_stage * StageInfo<PLAN>::BYTES, regs, ColSeq());
-          else load_all_staged<PLAN>(cm, imgsm, ring + (size_t)c_stage * StageInfo<PLAN>::BYTES, regs, ColSeq());
+          if (with_nulls) load_all_staged_nulls<PLAN, RT>(rl, b, cm, imgsm, tile_start, sm, ring + (size_t)c_stage * stage_size<PLAN, RT>(rl), regs, ColSeq());
+          else load_all_staged<PLAN, RT>(rl, cm, imgsm, ring + (size_t)c_stage * stage_size<PLAN, RT>(rl), regs, ColSeq());
           // The rows of this tile are in registers now: release the stage.  The stage was read through the GENERIC proxy (ld.shared)
           // and will be refilled through the ASYNC proxy (cp.async.bulk): the mbarrier alone does not order the two (PTX ISA, "async
           // proxy": accesses to the same location across proxies need a cross-proxy fence).  Without the fence a refill can land
@@ -1396,6 +1433,10 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
 
       // ---- row at a time over registers: filter -> group -> accumulate -------------------------
       c_scanned += __popc(live);
+#if SD_EXP_SKIP_ROWS
+      fold_all<PLAN>(regs, exp_sink, ColSeq());
+      continue;
+#endif
       if (PLAN::MODE == MODE_PROJECT || PLAN::MODE == MODE_MUTATE) {
         // filter -> project: passing rows become fixed-width records; one atomic per warp per row slot
         constexpr int NP = PLAN::NPROJ > 0 ? PLAN::NPROJ : 1;
@@ -1497,6 +1538,15 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
               }
             }
           } else if (args.table_mode == TABLE_PRIVATE) {
+#if SD_EXP_SINK_GROUPS   // (diagnostic builds: the slots and the group are computed, the table is never touched)
+            exp_sink += (uint64_t)g;
+            if constexpr (NORD > 0) combine_plain<PLAN>(exp_acc, 1, sv);
+            else {
+#pragma unroll
+              for (int s = 0; s < NSLOT; s++) exp_acc[s] = slot_combine(PLAN::slot_op(s), exp_acc[s], sv[s]);
+            }
+            continue;
+#endif
             uint64_t* t = table + (size_t)g * NSLOT * THREADS + tid;
             if constexpr (NORD > 0) combine_plain<PLAN>(t, THREADS, sv);
             else {
@@ -1594,6 +1644,13 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
       if (lane == 0) my_partials[e] = v;
     }
   }
+#if SD_EXP_SKIP_ROWS || SD_EXP_SINK_GROUPS
+  {   // the sinks feed a store that (almost) never happens, so the work that fills them survives
+#pragma unroll
+    for (int s = 0; s < NSLOT; s++) exp_sink ^= exp_acc[s];
+    if (exp_sink == 0x5d5d5d5d5d5d5d5dull) args.counters[7] = exp_sink;
+  }
+#endif
   // metrics
   {
     unsigned long long a = n_scanned, p = n_passed;
@@ -1631,6 +1688,31 @@ __global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::M
   }
   if (is_last && tid == 0) *args.ticket = 0;
 }
+
+template <class PLAN>
+__global__ void __launch_bounds__(THREADS + (PLAN::STAGES > 0 ? 32 : 0), PLAN::MIN_CTAS) scan_aggregate_kernel(const ScanArgs args) {
+  scan_aggregate<PLAN, false>(args, RingArgs{});
+}
+
+// A dense group-by's staged-only variant also has a kernel for two CTAs per SM, launched when the launch's compact ring
+// (RingArgs), the private table and the image tables fit half the SM (sd_engine.cu launch_scan): 2 x 9 warps on the SM's
+// four register partitions need <= 96 registers per thread, a cap the one-CTA kernel must not pay (wide plans would spill).
+template <class PLAN>
+struct TwoCtaKernel {
+  static constexpr bool BUILT = PLAN::MODE == MODE_GROUPS && !PLAN::SLOW_PATHS && PLAN::STAGES > 0 && PLAN::REG_GROUPS == 0;
+};
+template <class PLAN>
+__global__ void __launch_bounds__(THREADS + 32, 2) scan_aggregate_kernel_2cta(const ScanArgs args, const RingArgs ring) {
+  scan_aggregate<PLAN, true>(args, ring);
+}
+#ifndef __CUDACC_RTC__
+// the two-CTA kernel of PLAN for the registry, or nullptr
+template <class PLAN>
+const void* two_cta_kernel() {
+  if constexpr (TwoCtaKernel<PLAN>::BUILT) return (const void*)&scan_aggregate_kernel_2cta<PLAN>;
+  else return nullptr;
+}
+#endif
 
 }  // namespace sd
 #endif

@@ -43,9 +43,9 @@ std::string plan_struct_name(const std::string& signature) {
   snprintf(b, sizeof(b), "Plan_%016llx", h);
   return b;
 }
-AotRegistrar::AotRegistrar(const char* signature, const void* func, size_t tile_smem, int staged, size_t stage_bytes) {
+AotRegistrar::AotRegistrar(const char* signature, const void* func, size_t tile_smem, int staged, size_t stage_bytes, const void* func2) {
   KernelEntry e;
-  e.signature = signature; e.func = func; e.drv_func = nullptr; e.tile_smem = (tile_smem + 15) & ~size_t(15); e.origin = "aot";
+  e.signature = signature; e.func = func; e.drv_func = nullptr; e.func2 = func2; e.tile_smem = (tile_smem + 15) & ~size_t(15); e.origin = "aot";
   e.staged = staged; e.stage_bytes = stage_bytes; e.name = plan_struct_name(e.signature);
   kernel_registry().push_back(e);
 }
